@@ -182,7 +182,8 @@ int xrs_ebbi_f32(const float *red, const float *swir, const float *tir, float *o
 /* The group-by: aggregation into an open-addressing
  * hash table of `cap` slots (power of two >= 1024; device arrays keys/count/s1/s2/vmin/vmax of
  * `cap` entries, initialised by xrs_zonal_hash_init).  keys[slot] is the zone id (int64 for
- * integer zones, the bit pattern of the float64 value for float zones; INT64_MIN = empty),
+ * integer zones, the bit pattern of the float64 value for float zones; INT64_MIN = empty, so an int64
+ * zone INT64_MIN is not counted here -- xrs_zonal_hash_run reports it),
  * s1/s2 are sums of (v - pivot) and (v - pivot)^2.  Every finite zone value present in the
  * raster gets a slot, also when none of its cells is valid (count 0).  *overflow (device
  * int) is set when the raster holds more than `cap` distinct zones.  row_len is the raster's
@@ -197,23 +198,25 @@ int xrs_zonal_hash_accumulate(const void *values, int values_dtype, const void *
                               xrs_stream_t s);
 
 /* The whole single-pass group-by behind one call, with no host round trip in the middle: samples the
- * pivot on the device (unless use_pivot_hint: row stripes must share one pivot), initialises the table,
- * accumulates, then compacts the used slots into `packed` (device, 3 + 6 * max_out doubles):
+ * pivot on the device (median of 4096 strided samples, unless use_pivot_hint: row stripes must share one
+ * pivot), initialises the table, accumulates, then compacts the used slots into `packed` (device,
+ * 4 + 6 * max_out doubles):
  *   packed[0] = used slots, packed[1] = table overflowed (grow `cap` and retry), packed[2] = pivot,
+ *   packed[3] = an int64 zone INT64_MIN (the empty key, not in the table) was met: compute it apart,
  *   then 6 rows of max_out: key bit patterns, count (int64 bit patterns), s1, s2, min, max, in any
  *   order.  Slots beyond max_out are dropped (packed[0] > max_out tells; read the table instead).
- * flags: 2 device ints of scratch.  Replaces the sort + per-zone reductions of zonal.py:280-332. */
+ * flags: 3 device ints of scratch.  Replaces the sort + per-zone reductions of zonal.py:280-332. */
 int xrs_zonal_hash_run(const void *values, int values_dtype, const void *zones, int zones_dtype, int64_t n,
                        int64_t row_len, int has_nodata, double nodata, int use_pivot_hint, double pivot_hint,
                        int64_t *keys, int64_t *count, double *s1, double *s2, double *vmin, double *vmax, int cap,
                        double *packed, int max_out, int *flags, xrs_stream_t s);
 
-/* Second pass for float64 rasters (numpy's two-pass variance, zonal.py:75-76 `ndarray.std / var`): the same
+/* Second pass (numpy's two-pass variance, zonal.py:75-76 `ndarray.std / var`): the same
  * streaming group-by over the table xrs_zonal_hash_run left behind -- `keys` as populated by the first pass,
  * read only -- with sums taken about `zone_pivots[slot]` (device, `cap` doubles: the zone's mean from the
  * first pass) instead of one global pivot, so that s2 / n - (s1 / n)^2 does not cancel.  count / s1 / s2 /
  * vmin / vmax: a second set of `cap`-entry accumulators (reset here); `packed` / `flags` as above
- * (packed[2] = 0).  values_dtype must be XRS_F64.  */
+ * (packed[2] = 0).  values_dtype XRS_F32 or XRS_F64.  */
 int xrs_zonal_hash_second_pass(const void *values, int values_dtype, const void *zones, int zones_dtype, int64_t n,
                                int64_t row_len, int has_nodata, double nodata, const int64_t *keys,
                                const double *zone_pivots, int64_t *count, double *s1, double *s2, double *vmin,
@@ -221,7 +224,8 @@ int xrs_zonal_hash_second_pass(const void *values, int values_dtype, const void 
 
 /* `majority` (zonal.py:56-68): counts (zone, value) pairs of float32 values / int32 zones into
  * a hash table (keys/count of `cap` entries, initialised with xrs_zonal_hash_init; key =
- * (zone << 32) | float32 bits of the value, -0.0 folded into +0.0).  The caller picks the most
+ * (zone << 32) | (float32 bits of the value ^ 0x7fc00000), -0.0 folded into +0.0; the XOR makes the
+ * empty key INT64_MIN stand for (zone INT32_MIN, a NaN), a pair never counted).  The caller picks the most
  * frequent value per zone (smallest value on ties). */
 int xrs_zonal_pair_count(const float *values, const int32_t *zones, int64_t n, int64_t row_len,
                          int has_nodata, double nodata, int64_t *keys, int64_t *count, int cap,

@@ -345,6 +345,16 @@ def reference_outputs():
     g["apply_ones.dem"] = zo
     for kh, kw in ((5, 5), (25, 25), (3, 7), (9, 3)):
         g["apply_ones.mean.%dx%d" % (kh, kw)] = focal._apply_numpy(zo, np.ones((kh, kw)), focal._calc_mean)
+
+    # the hotspots classification (focal.py:881-915 `_calc_hotspots_numpy`) on float32 z-scores within
+    # +-2048 ulps of +-each threshold, plus signed zeros, NaN and +-inf.  Numba compares the float32 |z|
+    # with the float64 literals in float64, which decides the class exactly at z = +-1.96f.
+    steps = np.arange(-2048, 2049, dtype=np.int32)
+    thr = np.array([1.29, 1.65, 1.96, 2.33, 2.58], dtype=np.float32)
+    near = (thr.view(np.int32)[:, None] + steps[None, :]).reshape(-1).view(np.float32)
+    hz = np.concatenate([near, -near, np.array([0.0, -0.0, np.nan, np.inf, -np.inf], np.float32)])
+    g["hotspots.classify.z"] = hz
+    g["hotspots.classify.out"] = focal._calc_hotspots_numpy(hz[None, :])[0]
     return g
 
 

@@ -244,8 +244,14 @@ def hotspots(data, kernel, nthreads=1):
     global_std = np.nanstd(d)
     if global_std == 0:
         raise ZeroDivisionError("Standard deviation of the input raster values is 0.")
-    z = (mean_array - global_mean) / global_std
-    az = np.abs(z)
+    return hotspots_classify((mean_array - global_mean) / global_std)
+
+
+def hotspots_classify(z):
+    """focal.py:881-915 `_calc_hotspots_numpy`: float32 z-scores -> int8 confidence.  Numba compares the
+    float32 |z| with the float64 literals in float64 (NumPy would compare in float32), hence the promotion."""
+    z = np.asarray(z, dtype=np.float32)
+    az = np.abs(z).astype(np.float64)
     with np.errstate(invalid="ignore"):
         p = np.where(az >= 2.33, 0.0099, np.where(az >= 1.65, 0.0495, np.where(az >= 1.29, 0.0985, 1.0)))
         conf = np.where((az > 2.58) & (p < 0.01), 99, np.where((az > 1.96) & (p < 0.05), 95,

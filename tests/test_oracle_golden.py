@@ -229,6 +229,16 @@ def test_hotspots_vs_reference(refout):
     assert set(np.unique(r["hotspots.out"])) - {0} != set()      # the fixture really has hot / cold cells
 
 
+def test_hotspots_classification_at_the_thresholds(refout):
+    """float32 z within +-2048 ulps of +-every threshold, signed zeros, NaN, +-inf: the reference compares
+    in float64, so z = +-1.96f (which is above 1.96) is +-95, not +-90."""
+    z, ref = refout["hotspots.classify.z"], refout["hotspots.classify.out"]
+    got = o.hotspots_classify(z)
+    assert got.dtype == np.int8
+    np.testing.assert_array_equal(got, ref)
+    assert ref[z == np.float32(1.96)] == 95 and ref[z == -np.float32(1.96)] == -95
+
+
 def test_crosstab_vs_reference(refout):
     r = refout
     for agg in ("count", "percentage"):

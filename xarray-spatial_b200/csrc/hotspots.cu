@@ -44,16 +44,18 @@ __global__ void __launch_bounds__(256) global_stats_kernel(const float *__restri
     }
 }
 
-// focal.py:881-915 `_calc_hotspots_numpy` on z = (mean - global_mean) / global_std, all float32
+// focal.py:881-915 `_calc_hotspots_numpy` on z = (mean - global_mean) / global_std in float32.  Numba
+// compares the float32 |z| with the float64 literals in float64, so this does too: in float32 the
+// threshold 1.96 rounds up to 1.96000003815, and z = 1.96f would be classified 90 instead of 95.
 __global__ void __launch_bounds__(256) hotspots_classify_kernel(const float *__restrict__ mean, int64_t n,
                                                                 float gmean, float gstd, signed char *out) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const float z = (mean[i] - gmean) / gstd;
-        const float az = fabsf(z);
-        float p = 1.0f;
-        if (az >= 2.33f) p = 0.0099f; else if (az >= 1.65f) p = 0.0495f; else if (az >= 1.29f) p = 0.0985f;
+        const double az = fabs((double)z);
+        double p = 1.0;
+        if (az >= 2.33) p = 0.0099; else if (az >= 1.65) p = 0.0495; else if (az >= 1.29) p = 0.0985;
         int conf = 0;
-        if (az > 2.58f && p < 0.01f) conf = 99; else if (az > 1.96f && p < 0.05f) conf = 95; else if (az > 1.65f && p < 0.1f) conf = 90;
+        if (az > 2.58 && p < 0.01) conf = 99; else if (az > 1.96 && p < 0.05) conf = 95; else if (az > 1.65 && p < 0.1) conf = 90;
         const int hc = z > 0.f ? 1 : (z < 0.f ? -1 : 0);
         out[i] = (signed char)(hc * conf);
     }

@@ -31,7 +31,7 @@ struct ZhArgs {
     double pivot;
     const double *pivot_ptr;   // when not NULL the pivot is read from device memory (xrs_zonal_hash_run)
     const double *zone_pivots; // when not NULL: one pivot per slot of the (already populated) global table --
-                               // the second pass of float64 rasters, sums about the zones' own means
+                               // the second pass, sums about the zones' own means
     int has_nodata;
     double nodata;
     long long *keys;
@@ -39,6 +39,8 @@ struct ZhArgs {
     double *s1, *s2, *vmin, *vmax;
     int cap;  // global slots, power of two
     int *overflow;
+    int *sentinel;  // when not NULL: set to 1 if an int64 zone equals the empty key (INT64_MIN), which the table
+                    // cannot hold -- the host computes that one zone on its own
 };
 
 __device__ __forceinline__ unsigned zh_hash(long long key) {
@@ -221,7 +223,7 @@ template <typename T> __device__ __forceinline__ ZhQuad<T> zh_load(const T *p, i
     return q;
 }
 
-// ZP: sums about per-zone pivots (a.zone_pivots; the float64 second pass) instead of the one global pivot
+// ZP: sums about per-zone pivots (a.zone_pivots; the second pass) instead of the one global pivot
 template <typename VT, typename ZT, bool ZP>
 __global__ void __launch_bounds__(kZhThreads, 3) zonal_hash_kernel(const __grid_constant__ ZhArgs a_in) {
     ZhArgs a = a_in;
@@ -393,6 +395,9 @@ __global__ void __launch_bounds__(kZhThreads, 3) zonal_hash_kernel(const __grid_
                         cur_z = zk;
                         have = (zk == zk);
                         cur_ok = zh_key<ZT>(zk, cur_key);
+                        if constexpr (sizeof(ZT) == 8 && ZT(0.5) == ZT(0)) {
+                            if (!cur_ok && a.sentinel != nullptr) *a.sentinel = 1;
+                        }
                         if constexpr (ZP) {
                             if (cur_ok) {
                                 const int ps = zh_find(a.keys, a.cap, cur_key);
@@ -457,9 +462,13 @@ __global__ void __launch_bounds__(kZhThreads, 3) zonal_hash_kernel(const __grid_
 // ----------------------------------------------------------------------------- majority
 // `majority` (zonal.py:56-68: np.unique(values, return_counts) -> the most frequent value, the
 // smallest one on ties) needs per-zone value histograms.  One pass counts (zone, value) PAIRS in
-// the same kind of hash table: key = (int32 zone id << 32) | float32 bit pattern of the value.
-// The host then picks, per zone, the value with the largest count.  Meant for categorical
+// the same kind of hash table: key = (int32 zone id << 32) | (float32 bit pattern of the value ^
+// kZpValueXor).  The XOR moves the empty key kZhEmpty = (INT32_MIN << 32) | 0 onto the pair (zone
+// INT32_MIN, quiet NaN), which is never counted; with the plain bit pattern it was the pair (INT32_MIN,
+// 0.0) -- the usual int32 nodata zone and a common value -- and that pair's counts landed in an "empty"
+// slot.  The host then picks, per zone, the value with the largest count.  Meant for categorical
 // value rasters (few distinct values per zone); `cap` bounds the number of distinct pairs.
+constexpr unsigned kZpValueXor = 0x7fc00000u;
 struct ZpArgs {
     const float *values;
     const int *zones;
@@ -496,7 +505,7 @@ __global__ void __launch_bounds__(kZhThreads) zonal_pair_kernel(const __grid_con
     unsigned c0 = 0u, c1 = 0u;
     bool last1 = false;      // the run used most recently is run 1
     auto merge = [&](int zone, float val, unsigned cnt) {
-        const long long key = ((long long)zone << 32) | (long long)__float_as_uint(val);
+        const long long key = ((long long)zone << 32) | (long long)(__float_as_uint(val) ^ kZpValueXor);
         int s = zh_slot(s_keys, kCap, key, 64);
         if (s >= 0) { atomicAdd(&s_cnt[s], cnt); return; }
         s = zh_slot(a.keys, a.cap, key, a.cap);
@@ -608,31 +617,43 @@ __global__ void zonal_hash_reset_kernel(unsigned long long *count, double *s1, d
 }
 
 // ---- one-call front end: pivot sampling, table compaction and header, all on the device ----------
-// mean of up to 4096 finite samples taken at a regular stride: a shift that keeps sum((v - p)^2)
-// well conditioned (any value works; it only has to be the same for every cell)
+// median of up to 4096 finite samples taken at a regular stride: a shift that keeps sum((v - p)^2)
+// well conditioned (any value works; it only has to be the same for every cell).  The median, not the
+// mean: one FLT_MAX-style nodata sentinel among the samples would move the mean to ~1e35, and every
+// ordinary zone would then lose its values to the rounding of v - p.
 template <typename VT>
 __global__ void __launch_bounds__(256) zonal_pivot_kernel(const VT *__restrict__ v, int64_t n, double *out) {
-    __shared__ double s_sum[256];
-    __shared__ unsigned s_cnt[256];
-    const int64_t samples = n < 4096 ? n : 4096;
-    const int64_t step = n / samples;
-    double acc = 0.0;
-    unsigned cnt = 0u;
-    for (int64_t i = threadIdx.x; i < samples; i += 256) {
-        const double x = (double)v[i * step];
-        if (fabs(x) <= 1.7976931348623157e308) { acc += x; cnt += 1u; }
-    }
-    s_sum[threadIdx.x] = acc;
-    s_cnt[threadIdx.x] = cnt;
+    constexpr int kS = 4096;
+    __shared__ double s_v[kS];
+    __shared__ unsigned s_cnt;
+    if (threadIdx.x == 0) s_cnt = 0u;
     __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if ((int)threadIdx.x < o) { s_sum[threadIdx.x] += s_sum[threadIdx.x + o]; s_cnt[threadIdx.x] += s_cnt[threadIdx.x + o]; }
-        __syncthreads();
+    const int64_t samples = n < kS ? n : kS;
+    const int64_t step = n / samples;
+    for (int i = threadIdx.x; i < kS; i += 256) {
+        const double x = i < samples ? (double)v[i * step] : INFINITY;
+        const bool fin = fabs(x) <= 1.7976931348623157e308;
+        s_v[i] = fin ? x : INFINITY;            // non-finite samples sort to the end
+        if (fin) atomicAdd(&s_cnt, 1u);
     }
-    if (threadIdx.x == 0) *out = s_cnt[0] ? s_sum[0] / (double)s_cnt[0] : 0.0;
+    __syncthreads();
+    for (int k = 2; k <= kS; k <<= 1) {         // bitonic sort, ascending
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = threadIdx.x; i < kS; i += 256) {
+                const int l = i ^ j;
+                if (l > i) {
+                    const double a = s_v[i], b = s_v[l];
+                    if (((i & k) == 0) == (a > b)) { s_v[i] = b; s_v[l] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+    if (threadIdx.x == 0) *out = s_cnt ? s_v[s_cnt / 2] : 0.0;
 }
 
-// used slots -> dense rows of `packed` (6 rows of max_out doubles after a 3-double header), any order
+// used slots -> dense rows of `packed` (6 rows of max_out doubles after a kZhHeader-double header), any order
+constexpr int kZhHeader = 4;
 __global__ void __launch_bounds__(256) zonal_compact_kernel(const long long *keys, const unsigned long long *count,
                                                             const double *s1, const double *s2, const double *vmin,
                                                             const double *vmax, int cap, double *packed, int max_out,
@@ -643,7 +664,7 @@ __global__ void __launch_bounds__(256) zonal_compact_kernel(const long long *key
     if (k == kZhEmpty) return;
     const int pos = atomicAdd(&flags[1], 1);
     if (pos >= max_out) return;
-    double *row = packed + 3;
+    double *row = packed + kZhHeader;
     row[pos] = __longlong_as_double(k);
     row[max_out + pos] = __longlong_as_double((long long)count[i]);
     row[2 * max_out + pos] = s1[i];
@@ -655,10 +676,12 @@ __global__ void zonal_header_kernel(double *packed, const int *flags, const doub
     packed[0] = (double)flags[1];   // used slots
     packed[1] = (double)flags[0];   // table overflow
     packed[2] = *pivot;
+    packed[3] = (double)flags[2];   // an INT64_MIN zone was met (not in the table)
 }
 __global__ void zonal_flags_kernel(int *flags, double *pivot_dev, double pivot_hint) {
     flags[0] = 0;
     flags[1] = 0;
+    flags[2] = 0;
     if (pivot_dev) *pivot_dev = pivot_hint;
 }
 
@@ -710,7 +733,7 @@ int xrs_zonal_hash_accumulate(const void *values, int values_dtype, const void *
     a.zone_pivots = nullptr;
     a.has_nodata = has_nodata; a.nodata = nodata;
     a.keys = (long long *)keys; a.count = (unsigned long long *)count; a.s1 = s1; a.s2 = s2; a.vmin = vmin;
-    a.vmax = vmax; a.cap = cap; a.overflow = overflow;
+    a.vmax = vmax; a.cap = cap; a.overflow = overflow; a.sentinel = nullptr;
     cudaStream_t st = (cudaStream_t)s;
     int rc;
 #define XRS_ZH(VT)                                                               \
@@ -750,7 +773,7 @@ int xrs_zonal_hash_run(const void *values, int values_dtype, const void *zones, 
     a.zone_pivots = nullptr;
     a.has_nodata = has_nodata; a.nodata = nodata;
     a.keys = (long long *)keys; a.count = (unsigned long long *)count; a.s1 = s1; a.s2 = s2; a.vmin = vmin;
-    a.vmax = vmax; a.cap = cap; a.overflow = flags;
+    a.vmax = vmax; a.cap = cap; a.overflow = flags; a.sentinel = flags + 2;
     int rc;
 #define XRS_ZH(VT)                                                               \
     switch (zones_dtype) {                                                       \
@@ -775,7 +798,7 @@ int xrs_zonal_hash_second_pass(const void *values, int values_dtype, const void 
                                double *vmax, int cap, double *packed, int max_out, int *flags, xrs_stream_t s) {
     XRS_REQUIRE(values && zones && keys && zone_pivots && count && s1 && s2 && vmin && vmax && packed && flags,
                 "NULL pointer");
-    XRS_REQUIRE(values_dtype == XRS_F64, "the second pass is for float64 values");
+    XRS_REQUIRE(values_dtype == XRS_F32 || values_dtype == XRS_F64, "values must be float32 or float64");
     XRS_REQUIRE(zones_dtype >= XRS_F32 && zones_dtype <= XRS_I64, "unknown zones dtype");
     XRS_REQUIRE(cap >= 1024 && (cap & (cap - 1)) == 0, "cap must be a power of two >= 1024");
     XRS_REQUIRE(max_out >= 1, "max_out must be positive");
@@ -791,14 +814,17 @@ int xrs_zonal_hash_second_pass(const void *values, int values_dtype, const void 
     a.has_nodata = has_nodata; a.nodata = nodata;
     a.keys = (long long *)keys;   // every key of this raster is already in the table: find-or-insert only finds
     a.count = (unsigned long long *)count; a.s1 = s1; a.s2 = s2; a.vmin = vmin; a.vmax = vmax; a.cap = cap;
-    a.overflow = flags;
+    a.overflow = flags; a.sentinel = nullptr;
     int rc;
-    switch (zones_dtype) {
-        case XRS_I32: rc = launch_zh<double, int, true>(a, st); break;
-        case XRS_I64: rc = launch_zh<double, long long, true>(a, st); break;
-        case XRS_F32: rc = launch_zh<double, float, true>(a, st); break;
-        default: rc = launch_zh<double, double, true>(a, st); break;
+#define XRS_ZH(VT)                                                               \
+    switch (zones_dtype) {                                                       \
+        case XRS_I32: rc = launch_zh<VT, int, true>(a, st); break;               \
+        case XRS_I64: rc = launch_zh<VT, long long, true>(a, st); break;         \
+        case XRS_F32: rc = launch_zh<VT, float, true>(a, st); break;             \
+        default: rc = launch_zh<VT, double, true>(a, st); break;                 \
     }
+    if (values_dtype == XRS_F32) { XRS_ZH(float) } else { XRS_ZH(double) }
+#undef XRS_ZH
     if (rc != XRS_OK) return rc;
     zonal_compact_kernel<<<(cap + 255) / 256, 256, 0, st>>>((const long long *)keys, (const unsigned long long *)count,
                                                            s1, s2, vmin, vmax, cap, packed, max_out, flags);

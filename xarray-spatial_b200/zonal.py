@@ -43,14 +43,14 @@ _EMPTY_KEY = -(1 << 63)
 
 
 def _sample_pivot(values_t, comm=None):
-    """One global shift p keeps sum((v-p)^2) well conditioned; the mean of a small strided sample
-    is enough (one tiny device-to-host copy)."""
+    """One global shift p keeps sum((v-p)^2) well conditioned; the median of a small strided sample
+    is enough (one tiny device-to-host copy), and unlike the mean it ignores huge nodata sentinels."""
     import torch
     flat = values_t.reshape(-1)
     step = max(1, flat.numel() // 4096)
     sample = flat[::step][:4096].to(torch.float64).cpu().numpy()
     sample = sample[np.isfinite(sample)]
-    p0 = float(sample.mean()) if sample.size else 0.0
+    p0 = float(np.sort(sample)[sample.size // 2]) if sample.size else 0.0   # the device kernel's median
     if comm is not None:
         import torch.distributed as dist
         pt = torch.tensor([p0], dtype=torch.float64, device=values_t.device)
@@ -60,12 +60,28 @@ def _sample_pivot(values_t, comm=None):
 
 
 _MAX_OUT = 4096     # zones returned by the one-copy fast path of hash_partials
+_HDR = 4            # header doubles of the packed result: used slots, overflow, pivot, INT64_MIN zone met
+
+
+def _sentinel_partials(zones_t, values_t, nodata_values, pivot):
+    """Partials of the zone INT64_MIN, which the device table cannot hold (its key is the table's empty
+    key; the kernel only reports that it met the zone), by masked reductions over the raster."""
+    import torch
+    v = values_t.reshape(-1)
+    ok = (zones_t.reshape(-1) == -(1 << 63)) & torch.isfinite(v)
+    if nodata_values is not None:
+        ok &= v != nodata_values
+    vv = v[ok]
+    d = vv.to(torch.float64) - pivot
+    n = int(vv.numel())
+    return dict(count=np.array([n], np.int64), s1=np.array([float(d.sum())]), s2=np.array([float((d * d).sum())]),
+                min=np.array([float(vv.min()) if n else np.inf]), max=np.array([float(vv.max()) if n else -np.inf]))
 
 
 def hash_partials(zones_t, values_t, nodata_values=None, comm=None, cap=1 << 16, table=None):
     """One streaming pass that discovers the zone ids and accumulates their partials
     (xrs_zonal_hash_run: pivot sampling, table init, accumulation and compaction are enqueued
-    back to back; ONE device-to-host copy -- a 3-double header + 6 x 4096 doubles -- is the only
+    back to back; ONE device-to-host copy -- a 4-double header + 6 x 4096 doubles -- is the only
     synchronisation).  Returns (ids, part, pivot): ids = sorted unique finite zone values present
     in the raster (numpy, in the zones dtype), part = dict of numpy arrays aligned with ids
     (count int64; s1, s2, min, max float64), pivot = the scalar shift of s1/s2.
@@ -83,8 +99,8 @@ def hash_partials(zones_t, values_t, nodata_values=None, comm=None, cap=1 << 16,
     while True:
         # one blob: rows = keys, count (int64 bit patterns), s1, s2, min, max
         blob = torch.empty((6, cap), dtype=torch.float64, device=dev)
-        packed = torch.empty(3 + 6 * _MAX_OUT, dtype=torch.float64, device=dev)
-        flags = torch.empty(2, dtype=torch.int32, device=dev)
+        packed = torch.empty(_HDR + 6 * _MAX_OUT, dtype=torch.float64, device=dev)
+        flags = torch.empty(3, dtype=torch.int32, device=dev)
         keys, count = blob[0].view(torch.int64), blob[1].view(torch.int64)
         with torch.cuda.device(dev):
             _lib.call("xrs_zonal_hash_run", P(values_t), _dtype_code(values_t), P(zones_t), _dtype_code(zones_t),
@@ -94,14 +110,14 @@ def hash_partials(zones_t, values_t, nodata_values=None, comm=None, cap=1 << 16,
                       P(keys), P(count), P(blob[2]), P(blob[3]), P(blob[4]), P(blob[5]), cap,
                       P(packed), _MAX_OUT, P(flags), stream_ptr(values_t))
         host = packed.cpu().numpy()                    # the one synchronising copy
-        n_used, overflow, pivot = int(host[0]), int(host[1]), float(host[2])
+        n_used, overflow, pivot, sentinel = int(host[0]), int(host[1]), float(host[2]), int(host[3])
         if overflow == 0:
             break
         if cap >= (1 << 24):
             raise NotImplementedError("more than 16M distinct zones are not supported")
         cap *= 16
     if n_used <= _MAX_OUT:
-        rows = host[3:].reshape(6, _MAX_OUT)[:, :n_used]
+        rows = host[_HDR:].reshape(6, _MAX_OUT)[:, :n_used]
     else:                                               # many zones: gather the used slots of the table itself
         used = torch.nonzero(keys != _EMPTY_KEY).reshape(-1)
         rows = blob[:, used].cpu().numpy()
@@ -109,6 +125,10 @@ def hash_partials(zones_t, values_t, nodata_values=None, comm=None, cap=1 << 16,
     part = dict(count=np.ascontiguousarray(rows[1]).view(np.int64).copy(), s1=rows[2].copy(), s2=rows[3].copy(),
                 min=rows[4].copy(), max=rows[5].copy())
     ids = _keys_to_ids(k, zones_t.dtype)
+    if sentinel:
+        ids = np.append(ids, np.int64(_EMPTY_KEY))
+        sp = _sentinel_partials(zones_t, values_t, nodata_values, pivot)
+        part = {n: np.append(a, sp[n]) for n, a in part.items()}
     if table is not None:
         table.update(keys=keys, cap=cap)
     if comm is not None:
@@ -126,7 +146,7 @@ def _keys_to_ids(k, zones_dtype):
 
 
 def second_pass_partials(zones_t, values_t, table, ids, means, nodata_values=None, comm=None):
-    """numpy's two-pass variance for float64 rasters: a second streaming pass over the hash table
+    """numpy's two-pass variance: a second streaming pass over the hash table
     `hash_partials(..., table=...)` left on the device, with the sums taken about every zone's own
     mean (xrs_zonal_hash_second_pass; the means are scattered to the table's slots on the device, no
     host round trip beyond the one the first pass needed).  `ids`: sorted zone ids (numpy), `means`:
@@ -146,8 +166,8 @@ def second_pass_partials(zones_t, values_t, table, ids, means, nodata_values=Non
         idx = torch.searchsorted(ids_t, slot_ids).clamp_(max=nz - 1)
         pivots = means_t[idx].contiguous()                 # empty slots get some zone's mean: never read
         blob = torch.empty((5, cap), dtype=torch.float64, device=dev)
-        packed = torch.empty(3 + 6 * _MAX_OUT, dtype=torch.float64, device=dev)
-        flags = torch.empty(2, dtype=torch.int32, device=dev)
+        packed = torch.empty(_HDR + 6 * _MAX_OUT, dtype=torch.float64, device=dev)
+        flags = torch.empty(3, dtype=torch.int32, device=dev)
         count = blob[0].view(torch.int64)
         P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
         with torch.cuda.device(dev):
@@ -159,7 +179,7 @@ def second_pass_partials(zones_t, values_t, table, ids, means, nodata_values=Non
         host = packed.cpu().numpy()
         n_used = int(host[0])
         if n_used <= _MAX_OUT:
-            rows = host[3:].reshape(6, _MAX_OUT)[:, :n_used]
+            rows = host[_HDR:].reshape(6, _MAX_OUT)[:, :n_used]
         else:
             used = torch.nonzero(keys != _EMPTY_KEY).reshape(-1)
             rows = torch.cat([keys[used].view(torch.float64)[None], blob[:, used]]).cpu().numpy()
@@ -168,6 +188,10 @@ def second_pass_partials(zones_t, values_t, table, ids, means, nodata_values=Non
         part["count"][pos] = np.ascontiguousarray(rows[1]).view(np.int64)
         for i, n in enumerate(("s1", "s2", "min", "max")):
             part[n][pos] = rows[2 + i]
+        if not fz and ids[0] == _EMPTY_KEY:            # sorted ids: the INT64_MIN zone comes first
+            sp = _sentinel_partials(zones_t, values_t, nodata_values, float(means[0]))
+            for n in part:
+                part[n][0] = sp[n][0]
     if comm is not None and nz:
         import torch.distributed as dist
         t = {n: torch.as_tensor(a, device=dev) for n, a in part.items()}
@@ -178,6 +202,11 @@ def second_pass_partials(zones_t, values_t, table, ids, means, nodata_values=Non
         dist.all_reduce(t["max"], op=dist.ReduceOp.MAX, group=comm)
         part = {n: v.cpu().numpy() for n, v in t.items()}
     return part
+
+
+# the pair key's value half is the float32 bit pattern XOR this (csrc/zonal_hash.cu kZpValueXor): the
+# table's empty key then stands for (zone INT32_MIN, a NaN), a pair that is never counted
+_PAIR_VALUE_XOR = 0x7FC00000
 
 
 class _PairTableOverflow(Exception):
@@ -238,7 +267,7 @@ def pair_counts(zones_t, values_t, nodata_values=None, comm=None, cap=1 << 20, m
         k, inv = np.unique(k, return_inverse=True)
         c = np.bincount(inv, weights=c).astype(np.int64)
     zone = (k >> 32).astype(np.int64)
-    val = (k & 0xFFFFFFFF).astype(np.uint32).view(np.float32).astype(np.float64)
+    val = ((k & 0xFFFFFFFF) ^ _PAIR_VALUE_XOR).astype(np.uint32).view(np.float32).astype(np.float64)
     return zone, val, c
 
 
@@ -321,13 +350,23 @@ def majority_by_zone(zones_t, values_t, unique_zones, nodata_values=None, comm=N
     ok = torch.isfinite(v)
     if nodata_values is not None:
         ok &= v != float(nodata_values)
-    ids_t = torch.as_tensor(uz.astype(np.float64), device=z.device)
-    zf = z.to(torch.float64)
-    if z.dtype.is_floating_point:
-        ok &= torch.isfinite(z)
-    idx = torch.searchsorted(ids_t, zf).clamp_(max=len(uz) - 1)
-    ok &= ids_t[idx] == zf
+    idx, hit = _zone_index(z, uz)
+    ok &= hit
     return _majority_by_sort(idx[ok], v[ok], len(uz))
+
+
+def _zone_index(z, sel):
+    """(position in the sorted ids `sel`, cell's zone is in `sel`) for every cell of the flat zones `z`.
+    Integer ids are matched as int64: float64 would merge ids above 2^53."""
+    import torch
+    if z.dtype.is_floating_point:
+        ids_t = torch.as_tensor(np.asarray(sel, dtype=np.float64), device=z.device)
+        zk = z.to(torch.float64)
+    else:
+        ids_t = torch.as_tensor(np.asarray(sel, dtype=np.int64), device=z.device)
+        zk = z.to(torch.int64)
+    idx = torch.searchsorted(ids_t, zk).clamp_(max=len(sel) - 1)
+    return idx, ids_t[idx] == zk      # NaN zones match nothing
 
 
 def allreduce_tables(ids, part, dev, comm):
@@ -367,20 +406,50 @@ def allreduce_tables(ids, part, dev, comm):
     return union.astype(np.asarray(ids).dtype), {k: v.cpu().numpy() for k, v in dense.items()}
 
 
+# Bound on the relative error of the kernel's float64 sums (count, s1, s2 are each a float64 sum over a
+# zone's cells): 2^-40 = 8192 units in the last place, the worst case of a chain of 8192 roundings.
+_SUM_REL_ERR = 2.0 ** -40
+
+
+def one_pass_inaccurate(part, pivot):
+    """True when the partials about the one global `pivot` may miss the accuracy of numpy's two-pass
+    statistics (DESIGN 4.4).  With q = s2/n (mean square of v - pivot), the sums carry errors of about
+    e*sqrt(q) in s1/n and 3*e*q in s2/n - (s1/n)^2 (e = _SUM_REL_ERR).  The one-pass result is kept when
+    these stay ten times inside 1e-10 * (|mean| + M) for the mean and 1e-7 * var + 1e-12 * M^2 for the
+    variance, M being the zone's largest |value|; otherwise the caller sums again about each zone's mean."""
+    cnt = part["count"].astype(np.float64)
+    ok = (cnt > 0) & (part["min"] != part["max"])      # constant zones: finalize is exact for them
+    if not ok.any():
+        return False
+    n = cnt[ok]
+    m1 = part["s1"][ok] / n
+    q = part["s2"][ok] / n
+    var = np.maximum(q - m1 * m1, 0.0)
+    mean = pivot[ok] + m1 if np.ndim(pivot) else pivot + m1
+    big = np.maximum(np.abs(part["min"][ok]), np.abs(part["max"][ok]))
+    e = _SUM_REL_ERR
+    with np.errstate(over="ignore", invalid="ignore"):
+        bad_mean = e * np.sqrt(q) > 0.1 * 1e-10 * (np.abs(mean) + big)
+        bad_var = 3.0 * e * q > 0.1 * (1e-7 * var + 1e-12 * big * big)
+    return bool((bad_mean | bad_var).any())
+
+
 def finalize(part, pivot, stats_funcs):
     """dict stat -> float64 column; zones without valid cells are NaN (zonal.py:153-162)."""
     cnt = part["count"].astype(np.float64)
     ok = cnt > 0
+    const = part["min"] == part["max"]
     with np.errstate(invalid="ignore", divide="ignore"):
         m1 = part["s1"] / cnt
         cols = {}
         for s in stats_funcs:
+            # a zone whose valid values are all equal (min == max) gets numpy's exact mean, sum and var
             if s == "mean":
-                c = pivot + m1
+                c = np.where(const, part["min"], pivot + m1)
             elif s == "sum":
-                c = pivot * cnt + part["s1"]
+                c = np.where(const, part["min"] * cnt, pivot * cnt + part["s1"])
             elif s in ("var", "std"):
-                c = np.maximum(part["s2"] / cnt - m1 * m1, 0.0)
+                c = np.where(const, 0.0, np.maximum(part["s2"] / cnt - m1 * m1, 0.0))
                 if s == "std":
                     c = np.sqrt(c)
             elif s == "count":
@@ -418,24 +487,26 @@ def _stats_device(zones, values, zone_ids, stats_funcs, nodata_values, return_ty
         pos = np.searchsorted(unique_zones, sel)
         part = {n: a[pos] for n, a in part_all.items()}
     pivot = np.full(len(sel), pivot0)
-    cols = finalize(part, pivot, [s for s in names if s not in ("std", "var", "majority")])
+    # mean / sum / std / var come from a second pass about each zone's own mean (numpy's two-pass
+    # statistics) for float64 rasters when std / var are asked for, and for float32 rasters when the
+    # one-pass sums about the global pivot may be too inaccurate (zones far from the pivot for their spread)
+    sv = [s for s in names if s in ("std", "var")]
+    moments = [s for s in names if s in ("mean", "sum", "std", "var")]
+    second = len(sel) > 0 and bool(moments) and \
+        ((vt.dtype == torch.float64 and bool(sv)) or one_pass_inaccurate(part, pivot))
+    cols = finalize(part, pivot, [s for s in names if s != "majority" and not (second and s in moments)])
     if "majority" in names:
         maj = majority_by_zone(zt, vt, unique_zones, nodata_values, comm=comm)
         cols["majority"] = maj if zone_ids is None else maj[pos]
-    sv = [s for s in names if s in ("std", "var")]
-    if sv:
-        if vt.dtype == torch.float64 and len(sel):
-            # second pass about the per-zone means: numpy's two-pass variance, to ~1e-15
-            cnt = part_all["count"].astype(np.float64)
-            with np.errstate(invalid="ignore", divide="ignore"):
-                means = np.where(cnt > 0, pivot0 + part_all["s1"] / cnt, 0.0)
-            part2 = second_pass_partials(zt, vt, table, unique_zones, means, nodata_values, comm=comm)
-            if zone_ids is not None:
-                part2 = {n: a[pos] for n, a in part2.items()}
-                means = means[pos]
-            cols.update(finalize(part2, means, sv))
-        else:
-            cols.update(finalize(part, pivot, sv))
+    if second:
+        cnt = part_all["count"].astype(np.float64)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            means = np.where(cnt > 0, pivot0 + part_all["s1"] / cnt, 0.0)
+        part2 = second_pass_partials(zt, vt, table, unique_zones, means, nodata_values, comm=comm)
+        if zone_ids is not None:
+            part2 = {n: a[pos] for n, a in part2.items()}
+            means = means[pos]
+        cols.update(finalize(part2, means, moments))
     if return_type == 'pandas.DataFrame':
         d = {"zone": sel}
         for s in names:
@@ -452,10 +523,7 @@ def _broadcast_back(cols, names, sel, zt, shape, device):
     H, W = shape
     out = torch.full((len(names), H * W), float("nan"), dtype=torch.float64, device=device)
     if len(sel):
-        ids_t = torch.as_tensor(np.asarray(sel, dtype=np.float64), device=device)
-        zf = zt.reshape(-1).to(torch.float64)
-        idx = torch.searchsorted(ids_t, zf).clamp_(max=len(sel) - 1)
-        hit = ids_t[idx] == zf
+        idx, hit = _zone_index(zt.reshape(-1), sel)
         for i, s in enumerate(names):
             table = torch.as_tensor(np.asarray(cols[s], dtype=np.float64), device=device)
             out[i] = torch.where(hit, table[idx], out[i])
@@ -675,7 +743,8 @@ def _crosstab_3d(zones, values, zone_ids, cat_ids, layer, agg, nodata_values, co
         hit = (ids[pos] == sel) if len(ids) else np.zeros(len(sel), bool)
         if agg == "majority":
             col_all = majority_by_zone(zt, lt, ids, nodata_values, comm=comm)
-        elif agg in ("std", "var") and lt.dtype == torch.float64 and len(ids):
+        elif agg in ("mean", "sum", "std", "var") and len(ids) and \
+                ((lt.dtype == torch.float64 and agg in ("std", "var")) or one_pass_inaccurate(part, pivot0)):
             cnt = part["count"].astype(np.float64)
             with np.errstate(invalid="ignore", divide="ignore"):
                 means = np.where(cnt > 0, pivot0 + part["s1"] / cnt, 0.0)
