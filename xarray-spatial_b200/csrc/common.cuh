@@ -86,7 +86,7 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
         "l"(map), "r"(smem_u32(bar)), "r"(x), "r"(y)
         : "memory");
 }
-// same, with an L2 eviction-priority hint (0: evict_first for streamed inputs, 1: evict_last)
+// same, with an L2 eviction-priority hint (a policy from l2_policy_evict_first / l2_policy_evict_last)
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -103,6 +103,22 @@ __device__ __forceinline__ void tma_load_2d_hint(void *dst, const CUtensorMap *m
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
+// Bulk async store shared -> global (1-D, 16-byte aligned ends, size a multiple of 16), tracked by bulk groups.
+__device__ __forceinline__ void bulk_store(void *dst, const void *src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(src)),
+                 "r"(bytes)
+                 : "memory");
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed bulk group has finished READING shared memory (its global writes may still be in flight)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// generic-proxy writes to shared memory become visible to the async proxy (bulk copies)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 template <typename T> __device__ __forceinline__ T nan_of();
 template <> __device__ __forceinline__ float nan_of<float>() { return __int_as_float(0x7fc00000); }

@@ -31,26 +31,7 @@ static int launch_ingest(const void *in, int dtype, int64_t in_pitch, const type
     OutPtrs<Op> outs;
     outs.p[0] = out;
     outs.pitch_elems = out_pitch / 4;
-    constexpr int kPadS = SrcPad<TS>::value;
-    constexpr int kTileW = TileShape<WARPS, kPadS>::kTileW;
-    constexpr size_t smem = (size_t)STAGES * TileShape<WARPS, kPadS>::kNSub * ROWS * kSubW * sizeof(TS) +
-                            (size_t)2 * STAGES * sizeof(uint64_t);
-    auto kern = stencil3_tma_kernel<Op, ROWS, STAGES, WARPS, TS>;
-    XRS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, (WARPS + 1) * 32, smem));
-    if (per_sm < 1) per_sm = 1;
-    if (per_sm > CTAS) per_sm = CTAS;
-    const int64_t resident = (int64_t)sm_count() * per_sm;
-    const TileGeom g = make_tile_geom(H, W, kTileW, ROWS, resident);
-    const int64_t n_tasks = (int64_t)g.n_tiles * g.n_segs;
-    const int64_t grid = resident < n_tasks ? resident : n_tasks;
-    LaunchInfo &li = last_launch_info();
-    li.used_tma = 2;  // 2 = direct-ingest TMA kernel
-    li.grid = (int)grid; li.block = (WARPS + 1) * 32; li.smem_bytes = (int)smem;
-    kern<<<(unsigned)grid, (WARPS + 1) * 32, smem, stream>>>(tmap, prm, outs, g);
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    return launch_tma<Op, ROWS, STAGES, WARPS, CTAS, TS>(tmap, prm, outs, H, W, stream, 2);  // 2 = direct-ingest TMA kernel
 }
 
 // ring geometry: 2-byte cells need ROWS % 4 == 0 (128-byte aligned boxes); bytes in flight follow the

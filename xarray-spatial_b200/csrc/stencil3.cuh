@@ -21,7 +21,13 @@
 //     registers and combine them with the new row ("push, then emit the row above");
 //   * left / right neighbours are scalar shared-memory loads next to the lane's float4 (strip-edge
 //     lanes read the neighbouring strip or the tile halo: same addresses formula);
-//   * outputs are written as float4 with streaming stores.
+//   * outputs go the same way in reverse: consumer lanes put their float4 into a double-buffered
+//     shared-memory staging area (`out_full` / `out_empty` mbarriers), and ONE store warp writes
+//     each finished tile row with a single bulk async copy (cp.async.bulk), in raster order.  The
+//     earlier epilogue -- every warp storing its own 512 B per row at its own pace -- reached L2 as
+//     16 pieces per tile row at 16 different times, mixed into the read stream.  Operators whose
+//     staging does not fit next to the ring (the 4-output suite) keep the register stores, chosen
+//     at compile time (TmaCfg::kBulk).
 // Rasters TMA cannot describe (width not a multiple of 4 cells, unaligned base / pitch) run a
 // per-warp ring filled by cp.async (stencil3_cpasync_kernel); a plain bounds-checked direct-load
 // kernel is kept as the reference implementation of the loader.  All three drive the very same
@@ -125,6 +131,16 @@ template <typename TO> __device__ __forceinline__ void store4v(TO *p, const Vec4
     }
 }
 
+// 4 cells into the shared-memory output staging (16-byte aligned: one st.shared.v4 for f32)
+template <typename TO> __device__ __forceinline__ void store4_smem(TO *p, const Vec4<TO> &v) {
+    if constexpr (sizeof(TO) == 4) {
+        *reinterpret_cast<float4 *>(p) = make_float4(v.v[0], v.v[1], v.v[2], v.v[3]);
+    } else {
+        *reinterpret_cast<double2 *>(p) = make_double2(v.v[0], v.v[1]);
+        *reinterpret_cast<double2 *>(p + 2) = make_double2(v.v[2], v.v[3]);
+    }
+}
+
 // Operator concept (see surface_ops.cuh):
 //   using in_t = float|double;  static constexpr int kOutputs;  using out_t;
 //   struct Params;  __device__ Op(const Params&);
@@ -183,8 +199,25 @@ template <typename TI, typename TS> __device__ __forceinline__ void load_cells4_
     }
 }
 
-template <typename Op, int ROWS, int STAGES, int WARPS, typename TS = typename Op::in_t>
-__global__ void __launch_bounds__((WARPS + 1) * 32)
+// Shared-memory plan of one TMA-kernel instantiation: the input ring, then (bulk-store epilogue) kOutBufs
+// staging buffers of ROWS x kTileW cells per output, then the mbarriers.  The bulk epilogue is used when
+// CTAS such CTAs fit in an SM's 228 KB (1 KB of it reserved per CTA); otherwise lanes store from registers.
+constexpr size_t kSmemPerSm = 228 * 1024, kSmemPerCtaMax = 227 * 1024, kSmemReservedPerCta = 1024;
+constexpr int kOutBufs = 2;
+
+template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, typename TS = typename Op::in_t>
+struct TmaCfg {
+    static constexpr int kPadS = SrcPad<TS>::value;
+    static constexpr int kTileW = TileShape<WARPS, kPadS>::kTileW;
+    static constexpr size_t kRingBytes = (size_t)STAGES * TileShape<WARPS, kPadS>::kNSub * ROWS * kSubW * sizeof(TS);
+    static constexpr size_t kOutBufBytes = (size_t)ROWS * kTileW * Op::kOutputs * sizeof(typename Op::out_t);
+    static constexpr size_t kBulkSmem = kRingBytes + kOutBufs * kOutBufBytes + (2 * STAGES + 2 * kOutBufs) * sizeof(uint64_t);
+    static constexpr size_t kRegSmem = kRingBytes + 2 * STAGES * sizeof(uint64_t);
+    static constexpr bool kBulk = kBulkSmem <= kSmemPerCtaMax && CTAS * (kBulkSmem + kSmemReservedPerCta) <= kSmemPerSm;
+};
+
+template <typename Op, int ROWS, int STAGES, int WARPS, typename TS, bool BULK>
+__global__ void __launch_bounds__((WARPS + 1 + (BULK ? 1 : 0)) * 32)
 stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
                     const __grid_constant__ typename Op::Params prm,
                     const OutPtrs<Op> outs, const TileGeom g) {
@@ -198,12 +231,17 @@ stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
     constexpr int kBoxElems = ROWS * kSubW;
     constexpr int kStageElems = kNSub * kBoxElems;
     constexpr uint32_t kStageBytes = kStageElems * sizeof(T);
+    constexpr int kOutBufElems = BULK ? ROWS * kTileW * Op::kOutputs : 0;   // one staging buffer, [output][row][cell]
     static_assert((kBoxElems * sizeof(T)) % 128 == 0, "TMA destination must stay 128-byte aligned");
 
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     T *ring = reinterpret_cast<T *>(smem_raw);
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem_raw + (size_t)STAGES * kStageBytes);
+    TO *ostage = reinterpret_cast<TO *>(smem_raw + (size_t)STAGES * kStageBytes);
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem_raw + (size_t)STAGES * kStageBytes +
+                                                  (size_t)kOutBufs * kOutBufElems * sizeof(TO));
     uint64_t *empty = full + STAGES;
+    uint64_t *out_full = empty + STAGES;      // BULK only: WARPS arrivals, the staging buffer is written
+    uint64_t *out_empty = out_full + kOutBufs; // BULK only: one arrival, the bulk copies have read it
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
@@ -213,16 +251,65 @@ stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], WARPS);
         }
+        if constexpr (BULK) {
+#pragma unroll
+            for (int b = 0; b < kOutBufs; ++b) {
+                mbar_init(&out_full[b], WARPS);
+                mbar_init(&out_empty[b], 1);
+            }
+        }
         mbar_fence_init();
     }
     __syncthreads();
 
     const int64_t n_tasks = (int64_t)g.n_tiles * g.n_segs;
 
+    if (BULK && warp == WARPS + 1) {
+        // ---- store warp: one bulk copy per output row of the tile, in the consumers' (task, chunk) order
+        if (lane == 0) {
+            int ob = 0;
+            uint32_t phase = 0;  // bit b = parity to wait for on out_full[b]
+            for (int64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
+                const int seg = (int)(task / g.n_tiles), tile = (int)(task % g.n_tiles);
+                const int64_t y0 = (int64_t)seg * g.seg_rows;
+                const int seg_h = (int)(min(y0 + (int64_t)g.seg_rows, g.H) - y0);
+                const int n_chunks = (seg_h + 2 + ROWS - 1) / ROWS;
+                const int64_t x0 = (int64_t)tile * kTileW;
+                // W % 4 == 0 on this path: every row copy is a multiple of 16 bytes
+                const uint32_t bytes = (uint32_t)(min((int64_t)kTileW, g.W - x0) * (int64_t)sizeof(TO));
+                for (int c = 0; c < n_chunks; ++c) {
+                    mbar_wait(&out_full[ob], (phase >> ob) & 1u);
+                    phase ^= (1u << ob);
+                    const TO *src = ostage + ob * kOutBufElems;
+                    const int rel = c * ROWS - 2;  // output row (relative to y0) of the chunk's first row
+#pragma unroll
+                    for (int r = 0; r < ROWS; ++r) {
+                        if ((unsigned)(rel + r) >= (unsigned)seg_h) continue;  // lead-in rows / past the raster
+                        const int64_t off = (y0 + rel + r) * outs.pitch_elems + x0;
+#pragma unroll
+                        for (int k = 0; k < Op::kOutputs; ++k)
+                            if (Op::kOutputs == 1 || outs.p[k] != nullptr)
+                                bulk_store(outs.p[k] + off, src + (k * ROWS + r) * kTileW, bytes);
+                    }
+                    bulk_commit();
+                    bulk_wait_read_all();  // the staging buffer may be rewritten ...
+                    mbar_arrive(&out_empty[ob]);  // ... while its global writes drain
+                    ob = (ob + 1 == kOutBufs) ? 0 : ob + 1;
+                }
+            }
+            bulk_wait_read_all();
+        }
+        return;
+    }
+
     if (warp == WARPS) {
         // ---- producer: walks the same (task, chunk) sequence as the consumers, STAGES ahead
         if (lane == 0) {
             int stage = 0;
+            // Input lines are kept in L2 with evict_last priority, so the L2 evicts (writes back) the
+            // output lines first.  On an H100 this is 1.6 % faster than no hint for every 3x3 operator;
+            // evict_first on the loads is 3.5 % slower (DESIGN 4.1).
+            const uint64_t keep = l2_policy_evict_last();
             uint32_t phase = 0;  // bit s = parity of the `empty` phase stage s was last refilled under
             for (int64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
                 const int seg = (int)(task / g.n_tiles), tile = (int)(task % g.n_tiles);
@@ -238,7 +325,8 @@ stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
                     T *dst = ring + stage * kStageElems;
 #pragma unroll
                     for (int b = 0; b < kNSub; ++b)
-                        tma_load_2d(dst + b * kBoxElems, &tmap, &full[stage], bx + b * kSubW, by + c * ROWS);
+                        tma_load_2d_hint(dst + b * kBoxElems, &tmap, &full[stage], bx + b * kSubW, by + c * ROWS,
+                                         keep);
                     stage = (stage + 1 == STAGES) ? 0 : stage + 1;
                 }
             }
@@ -253,6 +341,9 @@ stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
     const int off_r = ((cc + kLaneCells) / kSubW) * kBoxElems + (cc + kLaneCells) % kSubW;
     int stage = 0;
     uint32_t phase = 0;  // bit s = parity to wait for on full[s]
+    int ob = 0;
+    uint32_t ophase = 0;  // BULK: bit b = parity of the out_empty phase buffer b was last written under
+    TO *const my_stage = ostage + kStripW * warp + kLaneCells * lane;   // BULK: this lane's cells, buffer 0, row 0
     for (int64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
         const int seg = (int)(task / g.n_tiles), tile = (int)(task % g.n_tiles);
         const int64_t y0 = (int64_t)seg * g.seg_rows;
@@ -264,14 +355,22 @@ stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
         const int64_t xl = (int64_t)tile * kTileW + kStripW * warp + kLaneCells * lane;
         const bool lane_ok = xl < g.W;  // W % 4 == 0 on this path: a lane is all-in or all-out
         const bool left_oob = xl == 0, right_oob = xl + 4 >= g.W;   // integer sources only
-        // output pointers one row above the first emitted row (y0 - 2): advanced before every store
+        // register stores: output pointers one row above the first emitted row (y0 - 2), advanced before every store
         TO *optr[Op::kOutputs];
+        if constexpr (!BULK) {
 #pragma unroll
-        for (int k = 0; k < Op::kOutputs; ++k) optr[k] = outs.p[k] + (y0 - 3) * outs.pitch_elems + xl;
+            for (int k = 0; k < Op::kOutputs; ++k) optr[k] = outs.p[k] + (y0 - 3) * outs.pitch_elems + xl;
+        }
 
         for (int c = 0; c < n_chunks; ++c) {
             mbar_wait(&full[stage], (phase >> stage) & 1u);
             phase ^= (1u << stage);
+            TO *ost = my_stage + ob * kOutBufElems;
+            if constexpr (BULK) {
+                // a fresh barrier passes a wait on parity 1: the first lap never blocks
+                mbar_wait(&out_empty[ob], ((ophase >> ob) & 1u) ^ 1u);
+                ophase ^= (1u << ob);
+            }
             const T *buf = ring + stage * kStageElems;
             const int rel = c * ROWS - 2;  // output row (relative to y0) of the stage's first row
             const int64_t ybase = y0 - 1 + (int64_t)c * ROWS;
@@ -294,16 +393,29 @@ stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
                 }
                 Vec4<TO> o[Op::kOutputs];
                 op.step(row, o);
-                const bool st = lane_ok && (unsigned)(rel + r) < (unsigned)seg_h;
+                if constexpr (BULK) {
+                    // every row goes to the staging buffer; the store warp copies only rows in [y0, y1)
+                    // and only the columns left of W
 #pragma unroll
-                for (int k = 0; k < Op::kOutputs; ++k) {
-                    optr[k] += outs.pitch_elems;
-                    if (st && (Op::kOutputs == 1 || outs.p[k] != nullptr)) store4v<TO>(optr[k], o[k]);
+                    for (int k = 0; k < Op::kOutputs; ++k)
+                        if (Op::kOutputs == 1 || outs.p[k] != nullptr) store4_smem<TO>(ost + (k * ROWS + r) * kTileW, o[k]);
+                } else {
+                    const bool st = lane_ok && (unsigned)(rel + r) < (unsigned)seg_h;
+#pragma unroll
+                    for (int k = 0; k < Op::kOutputs; ++k) {
+                        optr[k] += outs.pitch_elems;
+                        if (st && (Op::kOutputs == 1 || outs.p[k] != nullptr)) store4v<TO>(optr[k], o[k]);
+                    }
                 }
             }
-            __syncwarp();  // every lane is done reading this stage
-            if (lane == 0) mbar_arrive(&empty[stage]);
+            if constexpr (BULK) fence_proxy_async_smem();  // this lane's staging writes, visible to the bulk copies
+            __syncwarp();  // every lane is done reading this stage (and writing its staging cells)
+            if (lane == 0) {
+                mbar_arrive(&empty[stage]);
+                if constexpr (BULK) mbar_arrive(&out_full[ob]);
+            }
             stage = (stage + 1 == STAGES) ? 0 : stage + 1;
+            if constexpr (BULK) ob = (ob + 1 == kOutBufs) ? 0 : ob + 1;
         }
     }
 }
@@ -456,6 +568,8 @@ stencil3_cpasync_kernel(const typename Op::in_t *__restrict__ in, int64_t in_pit
 // segment height that minimises waves x (rows + lead-in rows a task streams), among heights of at least
 // `min_rows` with (rows + lead) a multiple of `quantum` (so the last chunk of a segment is full); among
 // heights within 1 % of the best prefer ~`want` waves (short tasks even out the partly filled last tile).
+// make_tile_geom asks for ~2 waves: at 32768^2 on an H100, long segments (fewer lead-in rows, fewer task
+// switches) were 0.4 % faster than ~8 waves for the 3x3 operators.
 inline int64_t pick_seg_rows(int64_t H, int64_t n_tiles, int64_t resident, int64_t min_rows, int64_t lead,
                              int64_t quantum, int64_t want) {
     if (H <= 0) return 1;
@@ -494,15 +608,45 @@ inline TileGeom make_tile_geom(int64_t H, int64_t W, int tile_w, int rows, int64
     g.H = H;
     g.W = W;
     g.n_tiles = (int)((W + tile_w - 1) / tile_w);
-    const int64_t seg_rows = pick_seg_rows(H, g.n_tiles, resident_ctas, 32, 2, rows, 8);
+    const int64_t seg_rows = pick_seg_rows(H, g.n_tiles, resident_ctas, 32, 2, rows, 2);
     g.seg_rows = (int)seg_rows;
     g.n_segs = (int)((H + seg_rows - 1) / seg_rows);
     return g;
 }
 
 // ROWS x STAGES = the TMA ring of the CTA-wide pipeline, WARPS consumer warps per CTA, CTAS CTAs per
-// SM: tuned per operator (scripts/tune/) -- ~65 KB in flight per SM
-// for the light operators, more warps and a deeper ring for the arithmetic-heavy ones.
+// SM: tuned per operator (surface.cu, scripts/tune/tune5.cu).  `kind` is what LaunchInfo::used_tma reports.
+// BULK defaults to the bulk-store epilogue wherever its staging fits; the tuning harness also times the
+// register-store epilogue.
+template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, typename TS = typename Op::in_t,
+          bool BULK = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, TS>::kBulk>
+int launch_tma(const CUtensorMap &tmap, const typename Op::Params &prm, const OutPtrs<Op> &outs, int64_t H,
+               int64_t W, cudaStream_t stream, int kind) {
+    using Cfg = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, TS>;
+    static_assert(!BULK || Cfg::kBulk, "the bulk-store staging does not fit next to this ring");
+    constexpr size_t smem = BULK ? Cfg::kBulkSmem : Cfg::kRegSmem;
+    constexpr int threads = (WARPS + 1 + (BULK ? 1 : 0)) * 32;  // consumers, producer[, store warp]
+    auto kern = stencil3_tma_kernel<Op, ROWS, STAGES, WARPS, TS, BULK>;
+    XRS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // persistent grid: CTAS per SM (or what fits), never more CTAs than tasks
+    int per_sm = 0;
+    XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > CTAS) per_sm = CTAS;
+    const int64_t resident = (int64_t)sm_count() * per_sm;
+    const TileGeom g = make_tile_geom(H, W, Cfg::kTileW, ROWS, resident);
+    const int64_t n_tasks = (int64_t)g.n_tiles * g.n_segs;
+    const int64_t grid = resident < n_tasks ? resident : n_tasks;
+    LaunchInfo &li = last_launch_info();
+    li.used_tma = kind;
+    li.grid = (int)grid;
+    li.block = threads;
+    li.smem_bytes = (int)smem;
+    kern<<<(unsigned)grid, threads, smem, stream>>>(tmap, prm, outs, g);
+    XRS_CUDA(cudaGetLastError());
+    return XRS_OK;
+}
+
 constexpr int kFallbackRows = 4, kFallbackStages = 4;  // cp.async ring (per warp)
 
 template <typename Op, int ROWS, int STAGES, int WARPS = 8, int CTAS = 2>
@@ -538,27 +682,8 @@ int launch_stencil3(const typename Op::in_t *in, int64_t in_pitch_bytes, const t
     CUtensorMap tmap;
     const bool tma_ok = out_vec_ok && (W % 4 == 0) &&
                         make_tensor_map_2d(&tmap, in, in_pitch_bytes, H, W, (int)sizeof(T), kSubW, ROWS);
-    if (tma_ok) {
-        constexpr int kTileW = TileShape<WARPS>::kTileW;
-        constexpr size_t smem = (size_t)STAGES * TileShape<WARPS>::kNSub * ROWS * kSubW * sizeof(T) +
-                                (size_t)2 * STAGES * sizeof(uint64_t);
-        auto kern = stencil3_tma_kernel<Op, ROWS, STAGES, WARPS>;
-        XRS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        // persistent grid: CTAS per SM (or what fits), never more CTAs than tasks
-        int per_sm = 0;
-        XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, (WARPS + 1) * 32, smem));
-        if (per_sm < 1) per_sm = 1;
-        if (per_sm > CTAS) per_sm = CTAS;
-        const int64_t resident = (int64_t)sms * per_sm;
-        const TileGeom g = make_tile_geom(H, W, kTileW, ROWS, resident);
-        const int64_t n_tasks = (int64_t)g.n_tiles * g.n_segs;
-        int64_t grid = resident < n_tasks ? resident : n_tasks;
-        li.used_tma = 1;
-        li.grid = (int)grid;
-        li.block = (WARPS + 1) * 32;
-        li.smem_bytes = (int)smem;
-        kern<<<(unsigned)grid, (WARPS + 1) * 32, smem, stream>>>(tmap, prm, outs, g);
-    } else {
+    if (tma_ok) return launch_tma<Op, ROWS, STAGES, WARPS, CTAS>(tmap, prm, outs, H, W, stream, 1);
+    {  // rasters TMA cannot describe: the per-warp cp.async ring
         constexpr int FR = sizeof(T) == 8 ? 2 : kFallbackRows, FS = kFallbackStages;
         StripGeom g;
         g.H = H;

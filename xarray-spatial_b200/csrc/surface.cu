@@ -7,19 +7,22 @@
 using namespace xrs;
 
 // Pipeline geometry per operator: ROWS rows per TMA stage, STAGES stages, WARPS consumer warps per CTA,
-// CTAs per SM (launch_stencil3), swept per operator with scripts/tune/tune4.cu: light operators want
-// ~65 KB in flight per SM and are indifferent to the warp count; slope / aspect need 16 consumer warps per
-// SM and a deeper ring to hide their arithmetic.  On an H100 SXM (400 W limit), 32768^2, slope, aspect,
-// curvature, hillshade, focal.mean, the 3x3 convolution and the fused suite all move 0.80-0.82 of the
-// 3.35 TB/s data-sheet HBM bandwidth (bench.py `ops`).
-#define XRS_CFG_LIGHT 2, 4, 16, 1     /* hillshade, curvature, focal.mean */
-#define XRS_CFG_CONV3 4, 4, 8, 1      /* 3x3 convolution */
-#define XRS_CFG_SLOPE_SQ 4, 3, 8, 2   /* slope, square cells */
-#define XRS_CFG_SLOPE 8, 2, 16, 1     /* slope, csx != csy */
-#define XRS_CFG_ASPECT 8, 2, 16, 1    /* aspect: arithmetic-bound */
-#define XRS_CFG_SUITE 8, 2, 12, 1     /* ~145 registers per thread: one 12-warp CTA per SM */
-#define XRS_CFG_F64 2, 4, 8, 1        /* 8-byte cells: focal.mean f64 */
-#define XRS_CFG_F32_F64 4, 4, 8, 1    /* float32 in, float64 out (12 B/cell) */
+// CTAs per SM (launch_stencil3), swept with scripts/tune/tune5.cu (output in tune5-h100.txt).  With the
+// bulk-store epilogue every single-output float32 operator is fastest, or within 0.3 % of it, at one
+// 16-warp CTA per SM with a 4 x 3 ring (100 KB of input in flight plus 64 KB of output staging); the
+// float64-output focal means prefer 2 x 4.  On an H100 80GB HBM3 (700 W limit), 32768^2, with the loads'
+// evict_last hint, these kernels move 0.84-0.85 of the 3.35 TB/s data sheet, 0.93-0.94 of the card's
+// measured cudaMemcpy rate (3039-3046 GB/s); focal.mean f64 moves 0.88 / 0.97.  The 4-output suite keeps the
+// register-store epilogue (its staging does not fit next to an 8 x 2 ring, and the smaller geometries where
+// it fits were not faster with it).
+#define XRS_CFG_LIGHT 4, 3, 16, 1     /* hillshade, curvature, focal.mean */
+#define XRS_CFG_CONV3 4, 3, 16, 1     /* 3x3 convolution */
+#define XRS_CFG_SLOPE_SQ 4, 3, 16, 1  /* slope, square cells */
+#define XRS_CFG_SLOPE 4, 3, 16, 1     /* slope, csx != csy */
+#define XRS_CFG_ASPECT 4, 3, 16, 1    /* aspect: the most arithmetic per cell */
+#define XRS_CFG_SUITE 8, 2, 12, 1     /* ~145 registers per thread: one 12-warp CTA per SM, register stores */
+#define XRS_CFG_F64 2, 4, 16, 1       /* 8-byte cells: focal.mean f64 */
+#define XRS_CFG_F32_F64 2, 4, 16, 1   /* float32 in, float64 out (12 B/cell) */
 
 static SlopeOp::Params slope_params(double cellsize_x, double cellsize_y) {
     const double kx = 1.0 / (8.0 * cellsize_x), ky = 1.0 / (8.0 * cellsize_y);
