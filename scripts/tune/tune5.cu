@@ -6,10 +6,16 @@
 //      cp.async.bulk per tile row issued by a store warp);
 //  (2) the flagship operators (square-cell slope, hillshade, focal.mean f32) over ROWS x STAGES x WARPS x
 //      CTAs per SM with both epilogues, then the other users of surface.cu's XRS_CFG_* geometries;
-//  (3) outputs of the two epilogues compared bit for bit at the shipped geometries.
+//  (1c) where the input boxes start: the shipped 32-byte halo (every box row starts on an L2 sector) against
+//      a 16-byte halo (every float32 box row starts 16 B into a sector), alternating, for the no-op operator and
+//      the flagship three and the 4-output suite; as the control, a float64 copy with its 32-byte halo read from an aligned base and
+//      from a base 16 B further on;
+//  (3) outputs of the two epilogues, and of the two halo widths, compared bit for bit at the shipped geometries.
 // Every line: CUDA-event median of 9 launches (after 2 warm-ups), GB/s of algorithmic bytes, fraction of
 // the 3.35 TB/s data sheet and of the best copy measured in (1).  nvidia-smi is sampled every 50 ms in the
 // background; each section prints the median SM clock and how many samples showed an active power cap.
+//
+// `tune5 align` runs (1), (1c) with 6 rounds instead of 3, and (3).
 //
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -fmad=false -DXRS_BUILD \
 //        -o tune5 scripts/tune/tune5.cu xarray-spatial_b200/csrc/lib_core.cu
@@ -136,18 +142,20 @@ __global__ void count_diff(const unsigned *a, const unsigned *b, size_t n, unsig
 }
 
 // The skeleton with nothing to compute: output row y-1 = input row y-1.
-struct CopyOp {
-    using in_t = float;
-    using out_t = float;
+template <typename T> struct CopyOpT {
+    using in_t = T;
+    using out_t = T;
     static constexpr int kOutputs = 1;
     struct Params { int unused; };
-    float r1[4];
-    __device__ explicit CopyOp(const Params &) { r1[0] = r1[1] = r1[2] = r1[3] = 0.f; }
-    __device__ __forceinline__ void step(const Row6<float> &row, Vec4<float> (&out)[1]) {
+    T r1[4];
+    __device__ explicit CopyOpT(const Params &) { r1[0] = r1[1] = r1[2] = r1[3] = T(0); }
+    __device__ __forceinline__ void step(const Row6<T> &row, Vec4<T> (&out)[1]) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) { out[0].v[i] = r1[i]; r1[i] = row.c[i]; }
     }
 };
+using CopyOp = CopyOpT<float>;
+using CopyOpD = CopyOpT<double>;
 
 static cudaEvent_t e0, e1;
 template <typename F> float time_it(F f, int reps = 9) {
@@ -162,23 +170,26 @@ template <typename F> float time_it(F f, int reps = 9) {
     return t[t.size() / 2];
 }
 
-// n/a codes: -1 does not fit (shared memory / occupancy below CTAS), -2 CUDA error, -3 no tensor map
-template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, bool BULK>
+// n/a codes: -1 does not fit (shared memory / occupancy below CTAS), -2 CUDA error, -3 no tensor map.
+// PAD = halo cells; `shift` > 0 reads the raster from `shift` cells past its base (W - 4 cells wide).
+template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, bool BULK, int PAD = SrcPad<typename Op::in_t>::value>
 float run(const typename Op::in_t *in, typename Op::out_t *const *outp, int64_t H, int64_t W,
-          const typename Op::Params &prm) {
+          const typename Op::Params &prm, int shift = 0) {
     using T = typename Op::in_t;
-    using Cfg = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS>;
+    using Cfg = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, T, PAD>;
     if constexpr (BULK && !Cfg::kBulk) {
         return -1.f;
     } else {
         CUtensorMap tmap;
-        if (!make_tensor_map_2d(&tmap, in, W * sizeof(T), H, W, sizeof(T), kSubW, ROWS)) return -3.f;
+        const int64_t pitch = W * sizeof(T);
+        if (shift) W -= 4;
+        if (!make_tensor_map_2d(&tmap, in + shift, pitch, H, W, sizeof(T), kSubW, ROWS)) return -3.f;
         OutPtrs<Op> outs;
         for (int k = 0; k < Op::kOutputs; ++k) outs.p[k] = outp[k];
-        outs.pitch_elems = W;
+        outs.pitch_elems = pitch / sizeof(T);
         constexpr size_t smem = BULK ? Cfg::kBulkSmem : Cfg::kRegSmem;
         constexpr int threads = (WARPS + 1 + (BULK ? 1 : 0)) * 32;
-        auto kern = stencil3_tma_kernel<Op, ROWS, STAGES, WARPS, T, BULK>;
+        auto kern = stencil3_tma_kernel<Op, ROWS, STAGES, WARPS, T, PAD, BULK>;
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
             cudaGetLastError();
             return -1.f;
@@ -186,7 +197,7 @@ float run(const typename Op::in_t *in, typename Op::out_t *const *outp, int64_t 
         int occ = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);
         if (occ < CTAS) return -1.f;
-        return time_it([&] { launch_tma<Op, ROWS, STAGES, WARPS, CTAS, T, BULK>(tmap, prm, outs, H, W, 0, 1); });
+        return time_it([&] { launch_tma<Op, ROWS, STAGES, WARPS, CTAS, T, PAD, BULK>(tmap, prm, outs, H, W, 0, 1); });
     }
 }
 
@@ -198,7 +209,8 @@ static void report(const char *name, const char *cfg, float ms, double bytes) {
     fflush(stdout);
 }
 
-int main() {
+int main(int argc, char **argv) {
+    const bool align_only = argc > 1 && strcmp(argv[1], "align") == 0;  // sections (1), (1c) and (3) only
     const int64_t H = 32768, W = 32768;
     const size_t n = (size_t)H * W;
     print_card();
@@ -243,6 +255,7 @@ int main() {
     AspectOp::Params ap = {0};
     CurvatureOp::Params cp = {100.0 / 900.0};
     CopyOp::Params np_ = {0};
+    CopyOpD::Params npd = {0};
     using FM = FocalMeanOp<float, float, false>;
     using FMD = FocalMeanOp<float, double, false>;
     using FDD = FocalMeanOp<double, double, false>;
@@ -272,35 +285,58 @@ int main() {
         BOTH(NAME, OP, in, o1, H, PRM, 8, 2, 16, 1, B8) BOTH(NAME, OP, in, o1, H, PRM, 8, 2, 8, 2, B8) \
         smi.summary(NAME, a, smi.mark()); }
 
-    // ---- (1b) the skeleton's copy operator, then (2) the flagship operators
-    SWEEP("copyop", CopyOp, np_)
-    SWEEP("slope(square)", SlopeSqOp, sp)
-    SWEEP("hillshade", HillshadeOp, hp)
-    SWEEP("focal.mean f32", FM, fp)
-
-    // ---- (2b) the other users of XRS_CFG_*
-#define OTHER(NAME, OP, IN, OUT, HH, PRM, BYTES) { size_t a = smi.mark(); \
-        BOTH(NAME, OP, IN, OUT, HH, PRM, 2, 4, 16, 1, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 3, 8, 2, BYTES) \
-        BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 4, 8, 1, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 3, 16, 1, BYTES) \
-        BOTH(NAME, OP, IN, OUT, HH, PRM, 2, 4, 8, 2, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 8, 2, 16, 1, BYTES) \
-        BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 2, 8, 2, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 2, 4, 8, 1, BYTES) \
-        smi.summary(NAME, a, smi.mark()); }
-    OTHER("slope(rxy)", SlopeOp, in, o1, H, sp2, B8)
-    OTHER("aspect", AspectOp, in, o1, H, ap, B8)
-    OTHER("curvature", CurvatureOp, in, o1, H, cp, B8)
-    OTHER("conv3", Conv3Op, in, o1, H, c3, B8)
-    OTHER("focal f32->f64", FMD, in, od1, H / 2, fdp, 12.0 * (n / 2))
-    OTHER("focal.mean f64", FDD, ind, od1, H / 2, fddp, 16.0 * (n / 2))
+    // ---- (1c) box alignment, alternating: 16-byte halo (PAD 4) against the shipped 32-byte halo (PAD 8),
+    //      shipped float32 geometry; float64 copy, shipped float64 geometry, from 32 B (sector-aligned) and 16 B past the base
     {
         size_t a = smi.mark();
-        BOTH("suite4", SuiteSqOp, in, o4, H, up, 8, 2, 12, 1, 20.0 * n)
-        BOTH("suite4", SuiteSqOp, in, o4, H, up, 2, 4, 8, 1, 20.0 * n)
-        BOTH("suite4", SuiteSqOp, in, o4, H, up, 2, 4, 12, 1, 20.0 * n)
-        BOTH("suite4", SuiteSqOp, in, o4, H, up, 4, 3, 8, 1, 20.0 * n)
-        BOTH("suite4", SuiteSqOp, in, o4, H, up, 2, 3, 16, 1, 20.0 * n)
-        BOTH("suite4", SuiteSqOp, in, o4, H, up, 4, 2, 12, 1, 20.0 * n)
-        smi.summary("suite4", a, smi.mark());
+        const double B16s = 16.0 * (H / 2) * (W - 4);
+#define ALIGN(NAME, OP, PRM) \
+        report(NAME, "halo 16 B bulk r4 s3 warps=16", run<OP, 4, 3, 16, 1, true, 4>(in, o1, H, W, PRM), B8); \
+        report(NAME, "halo 32 B bulk r4 s3 warps=16", run<OP, 4, 3, 16, 1, true, 8>(in, o1, H, W, PRM), B8);
+        for (int rep = 0; rep < (align_only ? 6 : 3); ++rep) {
+            ALIGN("copyop", CopyOp, np_)
+            ALIGN("slope(square)", SlopeSqOp, sp)
+            ALIGN("hillshade", HillshadeOp, hp)
+            ALIGN("focal.mean f32", FM, fp)
+            report("suite4", "halo 16 B reg  r8 s2 warps=12", run<SuiteSqOp, 8, 2, 12, 1, false, 4>(in, o4, H, W, up), 20.0 * n);
+            report("suite4", "halo 32 B reg  r8 s2 warps=12", run<SuiteSqOp, 8, 2, 12, 1, false, 8>(in, o4, H, W, up), 20.0 * n);
+            report("copyop f64", "base +32 B bulk r2 s4 warps=16", run<CopyOpD, 2, 4, 16, 1, true>(ind, od1, H / 2, W, npd, 4), B16s);
+            report("copyop f64", "base +16 B bulk r2 s4 warps=16", run<CopyOpD, 2, 4, 16, 1, true>(ind, od1, H / 2, W, npd, 2), B16s);
+        }
+        smi.summary("alignment", a, smi.mark());
     }
+
+    // ---- (1b) the skeleton's copy operator, then (2) the flagship operators
+    if (!align_only) {
+        SWEEP("copyop", CopyOp, np_)
+        SWEEP("slope(square)", SlopeSqOp, sp)
+        SWEEP("hillshade", HillshadeOp, hp)
+        SWEEP("focal.mean f32", FM, fp)
+
+        // ---- (2b) the other users of XRS_CFG_*
+#define OTHER(NAME, OP, IN, OUT, HH, PRM, BYTES) { size_t a = smi.mark(); \
+            BOTH(NAME, OP, IN, OUT, HH, PRM, 2, 4, 16, 1, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 3, 8, 2, BYTES) \
+            BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 4, 8, 1, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 3, 16, 1, BYTES) \
+            BOTH(NAME, OP, IN, OUT, HH, PRM, 2, 4, 8, 2, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 8, 2, 16, 1, BYTES) \
+            BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 2, 8, 2, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 2, 4, 8, 1, BYTES) \
+            smi.summary(NAME, a, smi.mark()); }
+        OTHER("slope(rxy)", SlopeOp, in, o1, H, sp2, B8)
+        OTHER("aspect", AspectOp, in, o1, H, ap, B8)
+        OTHER("curvature", CurvatureOp, in, o1, H, cp, B8)
+        OTHER("conv3", Conv3Op, in, o1, H, c3, B8)
+        OTHER("focal f32->f64", FMD, in, od1, H / 2, fdp, 12.0 * (n / 2))
+        OTHER("focal.mean f64", FDD, ind, od1, H / 2, fddp, 16.0 * (n / 2))
+        {
+            size_t a = smi.mark();
+            BOTH("suite4", SuiteSqOp, in, o4, H, up, 8, 2, 12, 1, 20.0 * n)
+            BOTH("suite4", SuiteSqOp, in, o4, H, up, 2, 4, 8, 1, 20.0 * n)
+            BOTH("suite4", SuiteSqOp, in, o4, H, up, 2, 4, 12, 1, 20.0 * n)
+            BOTH("suite4", SuiteSqOp, in, o4, H, up, 4, 3, 8, 1, 20.0 * n)
+            BOTH("suite4", SuiteSqOp, in, o4, H, up, 2, 3, 16, 1, 20.0 * n)
+            BOTH("suite4", SuiteSqOp, in, o4, H, up, 4, 2, 12, 1, 20.0 * n)
+            smi.summary("suite4", a, smi.mark());
+        }
+    }  // !align_only
 
     // ---- (3) the two epilogues agree bit for bit (shipped geometries)
     unsigned long long *cnt;
@@ -317,6 +353,18 @@ int main() {
     run<SlopeSqOp, 4, 3, 8, 2, false>(in, oref1, H, W, sp); run<SlopeSqOp, 4, 3, 8, 2, true>(in, o1, H, W, sp); diff("slope(square)");
     run<HillshadeOp, 2, 4, 16, 1, false>(in, oref1, H, W, hp); run<HillshadeOp, 2, 4, 16, 1, true>(in, o1, H, W, hp); diff("hillshade");
     run<FM, 2, 4, 16, 1, false>(in, oref1, H, W, fp); run<FM, 2, 4, 16, 1, true>(in, o1, H, W, fp); diff("focal.mean f32");
+    auto diffh = [&](const char *name) {
+        cudaMemset(cnt, 0, 8);
+        count_diff<<<132 * 8, 256>>>((const unsigned *)o[0], (const unsigned *)oref, n, cnt);
+        unsigned long long h = 0;
+        cudaMemcpy(&h, cnt, 8, cudaMemcpyDeviceToHost);
+        printf("16-byte vs 32-byte halo,   %-14s: %llu cells differ (%s)\n", name, h, cudaGetErrorString(cudaGetLastError()));
+        fflush(stdout);
+    };
+    cudaMemset(o[0], 0xff, n * 4); cudaMemset(oref, 0, n * 4);
+    run<SlopeSqOp, 4, 3, 16, 1, true, 4>(in, oref1, H, W, sp); run<SlopeSqOp, 4, 3, 16, 1, true, 8>(in, o1, H, W, sp); diffh("slope(square)");
+    run<HillshadeOp, 4, 3, 16, 1, true, 4>(in, oref1, H, W, hp); run<HillshadeOp, 4, 3, 16, 1, true, 8>(in, o1, H, W, hp); diffh("hillshade");
+    run<FM, 4, 3, 16, 1, true, 4>(in, oref1, H, W, fp); run<FM, 4, 3, 16, 1, true, 8>(in, o1, H, W, fp); diffh("focal.mean f32");
     smi.stop();
     return 0;
 }

@@ -16,7 +16,7 @@ bool make_tensor_map_2d_raw(CUtensorMap *map, const void *base, int64_t pitch_by
                             int dtype, int box_w, int box_h);  // lib_core.cu
 
 // The CTA-wide TMA pipeline of stencil3.cuh with a source element type TS != float: the ring holds the raw
-// cells (2-byte cells: 8-cell halos so that box starts stay 16-byte aligned), consumer lanes convert.
+// cells (32-byte halos, as for float32: 16 cells of 2 bytes, 8 of int32, 4 of float64), consumer lanes convert.
 template <typename Op, typename TS, int ROWS, int STAGES, int WARPS, int CTAS>
 static int launch_ingest(const void *in, int dtype, int64_t in_pitch, const typename Op::Params &prm, float *out,
                          int64_t out_pitch, int64_t H, int64_t W, cudaStream_t stream) {

@@ -6,7 +6,7 @@
 // a persistent CTA owns one (segment, tile) task at a time and marches down its rows.  Inside the
 // tile each consumer WARP owns a 128-cell strip and each lane 4 adjacent cells (one float4), so a
 // warp reads / writes 512 contiguous bytes per row.
-//   * ONE producer warp per CTA streams the tile (plus a 4-cell halo each side) through a ring of
+//   * ONE producer warp per CTA streams the tile (plus a 32-byte halo each side) through a ring of
 //     shared-memory stages with TMA 2-D boxes (208 cells x ROWS rows each; cp.async.bulk.tensor),
 //     `full` mbarriers carry the transaction bytes, `empty` mbarriers (one arrival per consumer
 //     warp) hand a stage back.  The producer is never delayed by arithmetic or stores, so the read
@@ -168,8 +168,12 @@ struct TileGeom {
 
 // Source element type TS of the raster in HBM (== the operator's input type for the plain kernels;
 // int16 / uint16 / int32 / float64 for direct ingestion, converted in registers with astype's
-// rounding).  The halo must keep the box start 16-byte aligned: 4 cells, 8 for 2-byte elements.
-template <typename TS> struct SrcPad { static constexpr int value = sizeof(TS) >= 4 ? 4 : 16 / (int)sizeof(TS); };
+// rounding).  The halo is 32 bytes (8 cells of 4 bytes, 16 of 2, 4 of 8): with an aligned raster every
+// box row then starts on a 32-byte L2 sector, and no sector is requested by two boxes.  With a 16-byte
+// halo every float32 box row started 16 B into a sector; slope, hillshade and focal.mean each took 2-3 %
+// longer on an H100 (DESIGN 4.1).  The pad must stay a multiple of 4 cells, so that a lane's 4 cells
+// never straddle two boxes (kSubW is one too).
+template <typename TS> struct SrcPad { static constexpr int value = 32 / (int)sizeof(TS); };
 
 template <int WARPS, int PAD = kPad> struct TileShape {
     static constexpr int kTileW = kStripW * WARPS;                       // output columns per CTA tile
@@ -205,9 +209,10 @@ template <typename TI, typename TS> __device__ __forceinline__ void load_cells4_
 constexpr size_t kSmemPerSm = 228 * 1024, kSmemPerCtaMax = 227 * 1024, kSmemReservedPerCta = 1024;
 constexpr int kOutBufs = 2;
 
-template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, typename TS = typename Op::in_t>
+template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, typename TS = typename Op::in_t,
+          int PAD = SrcPad<TS>::value>
 struct TmaCfg {
-    static constexpr int kPadS = SrcPad<TS>::value;
+    static constexpr int kPadS = PAD;
     static constexpr int kTileW = TileShape<WARPS, kPadS>::kTileW;
     static constexpr size_t kRingBytes = (size_t)STAGES * TileShape<WARPS, kPadS>::kNSub * ROWS * kSubW * sizeof(TS);
     static constexpr size_t kOutBufBytes = (size_t)ROWS * kTileW * Op::kOutputs * sizeof(typename Op::out_t);
@@ -216,7 +221,7 @@ struct TmaCfg {
     static constexpr bool kBulk = kBulkSmem <= kSmemPerCtaMax && CTAS * (kBulkSmem + kSmemReservedPerCta) <= kSmemPerSm;
 };
 
-template <typename Op, int ROWS, int STAGES, int WARPS, typename TS, bool BULK>
+template <typename Op, int ROWS, int STAGES, int WARPS, typename TS, int PAD, bool BULK>
 __global__ void __launch_bounds__((WARPS + 1 + (BULK ? 1 : 0)) * 32)
 stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
                     const __grid_constant__ typename Op::Params prm,
@@ -224,7 +229,8 @@ stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
     using TI = typename Op::in_t;   // what the operator consumes
     using T = TS;                   // what the ring holds
     using TO = typename Op::out_t;
-    constexpr int kPadS = SrcPad<TS>::value;
+    constexpr int kPadS = PAD;
+    static_assert(PAD % kLaneCells == 0 && kSubW % kLaneCells == 0, "a lane's cells must lie in one box");
     constexpr bool kIntegral = (TS(0.5) == TS(0));   // integer cells: the TMA unit zero-fills, NaN comes from coordinates
     constexpr int kTileW = TileShape<WARPS, kPadS>::kTileW;
     constexpr int kNSub = TileShape<WARPS, kPadS>::kNSub;
@@ -617,16 +623,16 @@ inline TileGeom make_tile_geom(int64_t H, int64_t W, int tile_w, int rows, int64
 // ROWS x STAGES = the TMA ring of the CTA-wide pipeline, WARPS consumer warps per CTA, CTAS CTAs per
 // SM: tuned per operator (surface.cu, scripts/tune/tune5.cu).  `kind` is what LaunchInfo::used_tma reports.
 // BULK defaults to the bulk-store epilogue wherever its staging fits; the tuning harness also times the
-// register-store epilogue.
+// register-store epilogue, and other halo widths PAD.
 template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, typename TS = typename Op::in_t,
-          bool BULK = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, TS>::kBulk>
+          int PAD = SrcPad<TS>::value, bool BULK = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, TS, PAD>::kBulk>
 int launch_tma(const CUtensorMap &tmap, const typename Op::Params &prm, const OutPtrs<Op> &outs, int64_t H,
                int64_t W, cudaStream_t stream, int kind) {
-    using Cfg = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, TS>;
+    using Cfg = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, TS, PAD>;
     static_assert(!BULK || Cfg::kBulk, "the bulk-store staging does not fit next to this ring");
     constexpr size_t smem = BULK ? Cfg::kBulkSmem : Cfg::kRegSmem;
     constexpr int threads = (WARPS + 1 + (BULK ? 1 : 0)) * 32;  // consumers, producer[, store warp]
-    auto kern = stencil3_tma_kernel<Op, ROWS, STAGES, WARPS, TS, BULK>;
+    auto kern = stencil3_tma_kernel<Op, ROWS, STAGES, WARPS, TS, PAD, BULK>;
     XRS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // persistent grid: CTAS per SM (or what fits), never more CTAs than tasks
     int per_sm = 0;
