@@ -109,6 +109,17 @@ def convolve_2d(data, kernel, nthreads=1):
     return out
 
 
+def convolve_2d_fma(data, kernel, nthreads=1):
+    """The CUDA convolve kernels' arithmetic: row-major taps, one fma(w, x, acc) per tap, out-of-raster taps
+    NaN.  Within float64 rounding of `convolve_2d`; the kernels equal it bit for bit."""
+    d = _f32(data)
+    k = np.ascontiguousarray(kernel, dtype=np.float64)
+    out = np.empty(d.shape, np.float32)
+    lib().xo_convolve2d_fma_f32(_p(d), _p(k), _int(k.shape[0]), _int(k.shape[1]), _p(out),
+                                _i64(d.shape[0]), _i64(d.shape[1]), _int(nthreads))
+    return out
+
+
 def focal_mean(data, passes=1, excludes=(np.nan,), nthreads=1):
     """focal.py:257-259 (astype(float) + passes loop) around `_mean_numpy` :44-67."""
     cur = np.ascontiguousarray(data, dtype=np.float64)

@@ -165,6 +165,28 @@ XO_EXPORT void xo_convolve2d_f32(const float *in, const double *kernel, int kh, 
     }
 }
 
+/* The project's CUDA convolve kernels restated: the same row-major tap order and +0.0 start, but every
+ * step is one fused multiply-add, acc = fma(w, (double)x, acc), and out-of-raster taps are NaN (so the
+ * border ring is NaN whatever the weights).  The GPU kernels must equal this bit for bit; it differs from
+ * xo_convolve2d_f32 (two roundings per tap) by float64 rounding only. */
+XO_EXPORT void xo_convolve2d_fma_f32(const float *in, const double *kernel, int kh, int kw,
+                                     float *out, int64_t H, int64_t W, int nthreads) {
+    const int ry = kh / 2, rx = kw / 2;
+#pragma omp parallel for num_threads(nthreads) schedule(static)
+    for (int64_t i = 0; i < H; ++i) {
+        for (int64_t j = 0; j < W; ++j) {
+            double acc = 0.0;
+            for (int ii = 0; ii < kh; ++ii)
+                for (int jj = 0; jj < kw; ++jj) {
+                    const int64_t y = i + ii - ry, x = j + jj - rx;
+                    const double v = (y >= 0 && y < H && x >= 0 && x < W) ? (double)in[y * W + x] : (double)NAN;
+                    acc = fma(kernel[ii * kw + jj], v, acc);
+                }
+            out[i * W + j] = (float)acc;
+        }
+    }
+}
+
 /* --------------------------------------------------------------- focal.mean
  * focal.py:44-67 `_mean_numpy` (one pass; focal.py:257-259 casts to float64 first and
  * loops passes).  Centre in `excludes` (NaN-aware equality, :37-41) -> copy; else

@@ -284,6 +284,7 @@ def test_focal_stats_multi_abi_ragged_width_falls_back_per_plane(xb):
               131 * 4, stride, 37, 131, kern.ctypes.data_as(ctypes.c_void_p), 3, 3, ids, 3,
               ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
     torch.cuda.synchronize()
+    assert used_tma(xb) == 8          # the bounds-checked single-statistic kernel served every plane
     for i, n in enumerate(names):
         got = buf[i * stride // 4: i * stride // 4 + 37 * 131].reshape(37, 131).cpu().numpy()
         assert_close_f32(got, o.focal_apply(z, kern, n, nthreads=4), what="multi fallback " + n)

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 import oracle as o
-from helpers import terrain
+from helpers import box_magnitude_fields, box_plant, box_planted_values, box_window_errors, terrain
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "xarray-spatial_b200", "csrc")
@@ -98,16 +98,26 @@ def test_compass_fold_matches_the_reference_branches():
         assert min(d, 360.0 - d) <= 1e-5 * abs(ref) + 1e-4, (X, Y, got, ref)
 
 
+def _box_threshold(z):
+    """NumPy statement of bs_threshold (box_stream.cu): 2^15 x the median |x| of the finite nonzero cells among
+    128 fixed sample cells (the upper median when their number is even); 2^100 when there is none."""
+    H, W = z.shape
+    s = np.arange(128)
+    a = np.abs(z[(2 * s + 1) * H // 256, (2 * ((79 * s) & 127) + 1) * W // 256].astype(np.float32))
+    a = np.sort(a[np.isfinite(a) & (a > 0)])
+    return np.float32(a[a.size // 2] * np.float32(32768.0)) if a.size else np.float32(2.0 ** 100)
+
+
 def _box_running(z, kh, kw, w, seg_rows=40):
     """NumPy statement of box_stream_kernel (box_stream.cu): per column a float64 RUNNING sum V of the
     last kh rows (add the entering row, emit, subtract the leaving row -- restarted every `seg_rows`
-    rows like the kernel's row segments), cells that are NaN / infinite / huge (|v| >= 2^100) kept out
-    of V and counted instead; horizontal window = difference of two inclusive prefixes of V; a window
-    holding a NaN is NaN, one holding an infinite / huge cell is re-summed tap by tap in the
-    reference's order, every other window is w * (running sum) + 0."""
+    rows like the kernel's row segments), exceptional cells (NaN, infinite, or |v| >= the launch's cut-off
+    `_box_threshold`) kept out of V and counted instead; horizontal window = difference of two inclusive
+    prefixes of V; a window holding a NaN is NaN, one holding an infinite / exceptional cell is re-summed tap
+    by tap in the reference's order, every other window is w * (running sum) + 0."""
     H, W = z.shape
     ry, rx = kh // 2, kw // 2
-    huge = np.float32(2.0 ** 100)
+    huge = _box_threshold(z)
     zp = np.full((H + 2 * ry, W + 2 * rx), np.nan, np.float32)       # TMA out-of-raster fill
     zp[ry:ry + H, rx:rx + W] = z
     isnan = np.isnan(zp)
@@ -136,12 +146,9 @@ def _box_running(z, kh, kw, w, seg_rows=40):
             res = (w * win + 0.0).astype(np.float32)
             nn, nb = Pn[x + kw] - Pn[x], Pb[x + kw] - Pb[x]
             res[nn > 0] = np.nan
-            for xx in np.nonzero((nn == 0) & (nb > 0))[0]:
-                acc = 0.0
-                with np.errstate(invalid="ignore", over="ignore"):
-                    for v in zp[y:y + kh, xx:xx + kw].astype(np.float64).ravel():
-                        acc = acc + w * v
-                    res[xx] = np.float32(acc)
+            redo = np.nonzero((nn == 0) & (nb > 0))[0]
+            if redo.size:                      # bs_direct: fma(w, v, acc) tap by tap
+                res[redo] = o.convolve_2d_fma(zp[y:y + kh], np.full((kh, kw), w))[ry, redo + rx]
             out[y] = res
             V = V - ordinary[y0 + r - (kh - 1)]
             Cn -= isnan[y0 + r - (kh - 1)]
@@ -163,13 +170,35 @@ def test_running_box_convolution_equals_tap_order_sums(kh, kw):
     dirty[56, 31] = np.float32(-3.4028235e38)
     for w in (1.0 / (kh * kw), -0.37):
         for data in (z, dirty):
-            ref = o.convolve_2d(data, np.full((kh, kw), w), nthreads=4)
+            ref = o.convolve_2d_fma(data, np.full((kh, kw), w), nthreads=4)   # the recompute's tap order
             got = _box_running(data, kh, kw, w)
             np.testing.assert_array_equal(np.isnan(got), np.isnan(ref))
             m = np.isfinite(ref) & (np.abs(ref) < 1e20)
             odd = ~m & ~np.isnan(ref)
             np.testing.assert_allclose(got[odd], ref[odd], rtol=1e-6)            # +-inf and huge windows
             np.testing.assert_allclose(got[m], ref[m], rtol=1e-6, atol=1e-6 * np.abs(ref[m]).max())
+
+
+@pytest.mark.parametrize("field", ["terrain", "offset", "lognormal"])
+@pytest.mark.parametrize("kh,kw", [(5, 5), (3, 9), (1, 7), (25, 25), (25, 3)])
+def test_running_box_is_not_contaminated_by_large_cells(kh, kw, field):
+    """A finite cell far above the data (a 1e20 fill value) must leave no rounding behind in the running column
+    sums: every window without a NaN / inf / planted cell stays within 2 ulp32 + 2^-36 |w| kh kw M of the
+    FMA-oracle's tap-order sum, for planted magnitudes from 2^24 M to FLT_MAX, both signs, single cells and
+    3-row runs, at the model's segment starts and within kh rows of the raster's top and bottom.  With the
+    former absolute 2^100 cut-off, 1e15 .. 1e29 entered V and left errors of up to the whole window."""
+    rng = np.random.default_rng(kh * 100 + kw)
+    H = 130
+    z = box_magnitude_fields(rng, H, 60)[field]
+    M = float(np.abs(z).max())
+    rows = [0, 1, kh // 2, 40, 41, 80, 120, H - 1 - kh // 2, H - 2, H - 1]
+    for value in box_planted_values(M):
+        data, planted = box_plant(z, value, rows, rng)
+        assert _box_threshold(data) <= 2.0 ** 15 * M
+        for w in (1.0 / (kh * kw), -0.37):
+            ref = o.convolve_2d_fma(data, np.full((kh, kw), w), nthreads=4)
+            got = _box_running(data, kh, kw, w)
+            box_window_errors(got, ref, planted, kh, kw, w, M, "%s %dx%d %g w=%g" % (field, kh, kw, value, w))
 
 
 def _lane_sum_windows(v, rx):

@@ -171,6 +171,47 @@ def test_convolve_vs_reference(refout, kn):
     np.testing.assert_array_equal(o.convolve_2d(refout["conv.dem_nan"], k), refout["conv.out_nan." + kn])
 
 
+def _fma_within_float64_rounding(data, k, what):
+    """convolve_2d_fma (one rounding per tap, the CUDA kernels' order) against convolve_2d (the reference's
+    num += w * x, two roundings per tap): identical NaN masks, and elsewhere
+    |a - b| <= ulp32(max(|a|, |b|)) + 2 n 2^-53 sum|w x| over the window, n = kh kw."""
+    from scipy.signal import correlate2d
+    a = o.convolve_2d_fma(data, k, nthreads=4)
+    b = o.convolve_2d(data, k, nthreads=4)
+    np.testing.assert_array_equal(np.isnan(a), np.isnan(b), err_msg=what + ": NaN masks differ")
+    inf = np.isinf(b)
+    np.testing.assert_array_equal(a[inf], b[inf], err_msg=what + ": infinite windows differ")
+    m = np.isfinite(b)
+    mag = correlate2d(np.nan_to_num(np.abs(data.astype(np.float64)), posinf=0.0), np.abs(k), mode="same")
+    n = k.size
+    big = np.maximum(np.abs(a[m]), np.abs(b[m]))
+    bound = np.spacing(big).astype(np.float64) + 2 * n * 2.0 ** -53 * mag[m]
+    err = np.abs(a[m].astype(np.float64) - b[m].astype(np.float64))
+    assert (err <= bound).all(), "%s: worst %.3g over the bound" % (what, (err / bound).max())
+
+
+@pytest.mark.parametrize("kn", ["box3", "box9", "mixed5", "mixed3x7", "mixed25", "int3"])
+def test_fma_convolve_oracle_on_the_goldens(refout, kn):
+    k = refout["conv.kernel." + kn]
+    for d in ("conv.dem", "conv.dem_nan"):
+        _fma_within_float64_rounding(refout[d], k, "%s %s" % (d, kn))
+
+
+@pytest.mark.parametrize("kh,kw", [(3, 3), (5, 5), (9, 9), (13, 13), (25, 25), (3, 5), (9, 5), (7, 1), (1, 31),
+                                   (63, 1), (49, 49)])
+def test_fma_convolve_oracle_at_kernel_shapes(kh, kw):
+    """The FMA oracle stays within float64 rounding of the reference's order for mixed and zero-tap weights,
+    on rasters smaller than, equal to and larger than the window, with magnitudes up to 1e6 + offsets."""
+    rng = np.random.default_rng(kh * 64 + kw)
+    for H, W in ((1, 4), (kh, kw + 3), (65, 132)):
+        z = (rng.standard_normal((H, W)).cumsum(1) * 50.0 + 1e6 * rng.random()).astype(np.float32)
+        z[rng.random((H, W)) < 0.01] = np.nan
+        mixed = rng.standard_normal((kh, kw)) * 0.3
+        zero_taps = np.where(rng.random((kh, kw)) < 0.4, 0.0, mixed)
+        for name, k in (("mixed", mixed), ("zero taps", zero_taps)):
+            _fma_within_float64_rounding(z, k, "%dx%d %s on %dx%d" % (kh, kw, name, H, W))
+
+
 @pytest.mark.parametrize("mn", ["circle3", "full3", "annulus5", "rect3x5", "weights3"])
 def test_focal_apply_vs_reference(refout, mn):
     for s in STATS:

@@ -30,11 +30,14 @@
 // Numerics.  The reference accumulates fma(w, v, acc) tap by tap in float64; here the window sum is
 // formed in float64 (sums of float32 cells: rounding ~1e-16 of the window's magnitude) and scaled
 // once -- far inside the 1e-5 bar of the float32 result.  Running sums are only trustworthy while
-// every cell that entered them is "ordinary": a cell that is NaN, infinite or huge (|v| >= 2^100,
-// e.g. a 3.4e38 nodata sentinel, which would wipe out the float64 low bits of V for as long as it
-// stays in the window and corrupt it for good when it leaves) is kept OUT of V and counted instead
-// (two 16-bit running counts per column, same lane-sum machinery): a window holding a NaN is NaN like
-// the reference's; a window holding an infinite / huge cell is recomputed tap by tap in the
+// every cell that entered them is "ordinary": a cell far larger than the data around it (a 1e20
+// fill value in a DEM: its float64 ulp is 16384) rounds away the low bits of every other cell of its
+// column while it is in V, and subtracting it later does not bring them back, so every later window of
+// that column would be wrong.  A cell is therefore EXCEPTIONAL when it is NaN, infinite or at least
+// 2^15 x the median |x| of a fixed 128-cell sample of the raster (bs_threshold: one cut-off per launch;
+// 2^100 when the sample holds no finite nonzero cell).  Exceptional cells are kept OUT of V and counted
+// instead (two 16-bit running counts per column, same lane-sum machinery): a window holding a NaN is NaN
+// like the reference's; a window holding an infinite / exceptional cell is recomputed tap by tap in the
 // reference's order from global memory; all other windows never saw the bad cell.  Batches without any
 // such cell -- one warp vote per 4 rows -- skip the masking and the counts entirely.
 #include "stencil3.cuh"
@@ -43,9 +46,47 @@ namespace xrs {
 
 constexpr int kBsWarps = 7;      // consumer warps per CTA (+ 1 producer warp)
 constexpr int kBsMaxK = 25;      // window rows / columns served
-constexpr float kBsHuge = 1.2676506e30f;  // 2^100: cells at or above stay out of the running sums
+constexpr float kBsHuge = 1.2676506e30f;  // 2^100: the cut-off when the sample holds no finite nonzero cell
+constexpr float kBsScale = 32768.f;       // 2^15: cells at or above kBsScale x the sample median are exceptional
 constexpr int kB2Rows = 4;       // rows per stage half (entering / leaving)
 constexpr int kBoxNotTaken = -12345;
+
+// The launch's cut-off between ordinary cells (summed into V) and exceptional ones (kept out of V, their windows
+// recomputed tap by tap): 2^15 x the median |x| of the finite nonzero cells among 128 fixed sample cells
+// (sample s = 4 lane + j at row (2 s + 1) H / 256, column (2 ((79 s) mod 128) + 1) W / 256).  Every warp of
+// every CTA computes the same value.  A median ignores a few planted sentinels, and a cut-off relative to the
+// data keeps any ordinary cell from rounding away more than ~2^-38 of the data's magnitude from a column sum
+// (DESIGN section 4.2).  Mirrored by `_box_threshold` in tests/test_kernel_algebra.py.
+__device__ __noinline__ float bs_threshold(const float *__restrict__ in, int64_t pitch_elems, int64_t H, int64_t W) {
+    const int lane = threadIdx.x & 31;
+    float a[4];
+    bool ok[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int s = 4 * lane + j;
+        const int64_t y = (2 * s + 1) * H / 256, x = (2 * ((79 * s) & 127) + 1) * W / 256;
+        a[j] = fabsf(in[y * pitch_elems + x]);
+        ok[j] = a[j] > 0.f && a[j] < __int_as_float(0x7f800000);   // NaN fails both
+    }
+    int rank[4] = {0, 0, 0, 0}, n = 0;
+    for (int src = 0; src < 32; ++src) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float b = __shfl_sync(0xffffffffu, a[k], src);
+            const bool okb = __shfl_sync(0xffffffffu, ok[k], src);
+            n += okb;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)   // order by (value, sample index): every rank 0 .. n - 1 is held once
+                rank[j] += okb && (b < a[j] || (b == a[j] && 4 * src + k < 4 * lane + j));
+        }
+    }
+    unsigned med = 0u;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+        if (ok[j] && rank[j] == n / 2) med = __float_as_uint(a[j]);
+    med = __reduce_max_sync(0xffffffffu, med);
+    return n ? __uint_as_float(med) * kBsScale : kBsHuge;
+}
 
 __device__ __noinline__ float bs_direct(const float *__restrict__ in, int64_t pitch_elems, int64_t H, int64_t W,
                                         int64_t y, int64_t x, int kh, int kw, double w) {
@@ -254,6 +295,7 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
     const int off = (col / S::kBoxW) * S::kBoxCells + (col % S::kBoxW);  // + i * kBoxW for row i of the half
     const bool emits = (4 * lane >= S::kPad) && (4 * lane < kStripW - S::kPad);
     const uint32_t win_mask = bs_bits(kh - 1);   // the rows in the window before a row is added
+    const float thr = bs_threshold(in, in_pitch_elems, g.H, g.W);
     int stage = 0;
     uint32_t lap = 0;
     for (int64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
@@ -308,7 +350,7 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
                 }
                 const float amax = bs_amax3(bs_amax3(bs_amax4(nv[0]), nv[1][0], nv[1][1]),
                                             bs_amax3(bs_amax4(nv[2]), nv[1][2], nv[1][3]), bs_amax4(nv[3]));
-                if (!__any_sync(0xffffffffu, watch && !(amax < kBsHuge))) {
+                if (!__any_sync(0xffffffffu, watch && !(amax < thr))) {
                     float ov[kB2Rows][4];
 #pragma unroll
                     for (int i = 0; i < kB2Rows; ++i) {
@@ -367,7 +409,7 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
                     const float4 q = *reinterpret_cast<const float4 *>(se + i * S::kBoxW);
                     const bool zero_lane = MODE == 1 && !in_raster;
                     const float v[4] = {zero_lane ? 0.f : q.x, zero_lane ? 0.f : q.y, zero_lane ? 0.f : q.z, zero_lane ? 0.f : q.w};
-                    const bool row_dirty = __any_sync(0xffffffffu, watch && !(bs_amax4(v) < kBsHuge));
+                    const bool row_dirty = __any_sync(0xffffffffu, watch && !(bs_amax4(v) < thr));
                     dirty = (dirty << 1) | (row_dirty ? 1u : 0u);
                     if (!row_dirty) {
 #pragma unroll
@@ -376,7 +418,7 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
                             const bool isnan_ = v[j] != v[j];
-                            const bool big = !isnan_ && !(fabsf(v[j]) < kBsHuge);
+                            const bool big = !isnan_ && !(fabsf(v[j]) < thr);
                             V[j] += (isnan_ || big) ? 0.0 : (double)v[j];
                             C[j] += isnan_ ? 1u : (big ? 0x10000u : 0u);
                         }
@@ -426,7 +468,7 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
                             const bool isnan_ = vo[j] != vo[j];
-                            const bool big = !isnan_ && !(fabsf(vo[j]) < kBsHuge);
+                            const bool big = !isnan_ && !(fabsf(vo[j]) < thr);
                             V[j] -= (isnan_ || big) ? 0.0 : (double)vo[j];
                             C[j] -= isnan_ ? 1u : (big ? 0x10000u : 0u);
                         }

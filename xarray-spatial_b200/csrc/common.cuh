@@ -16,7 +16,8 @@ int cuda_fail(cudaError_t e, const char *what);
 
 struct LaunchInfo {  // for tests / profiling: what the last launch on this thread chose
     int used_tma;    // 0 cp.async strip kernel, 1 TMA strip kernel, 2 direct-ingest, 3 running-box kernel,
-                     // 4 generic tiled convolve, 5 bounds-checked fallback
+                     // 4 generic tiled convolve, 5 bounds-checked convolve fallback, 6 fused focal statistics,
+                     // 7 tiled focal statistic, 8 bounds-checked focal statistic fallback
     int grid, block, smem_bytes;
 };
 LaunchInfo &last_launch_info();

@@ -301,6 +301,15 @@ conv2d_direct_kernel(const float *__restrict__ in, int64_t in_pitch_elems, const
 // Reducers follow Numba's nan-functions (numba/np/arraymath.py) as used by focal.py:268-302:
 // mean/var/std accumulate in f64 (var two-pass about the f64 mean), sum accumulates in f32 in
 // row-major window order (bit-identical to np.nansum on the f32 scratch), min/max skip NaN.
+// Numba's nanmin / nanmax step: replace unless strictly ordered, so a NaN accumulator takes the first
+// non-NaN cell, a NaN cell never replaces, and among equal cells (-0.0 and +0.0) the LAST in window order
+// wins.  fminf / fmaxf would differ in the sign bit: they order -0.0 below +0.0.
+__device__ __forceinline__ void nan_min_step(float &mn, float v) {
+    if (v == v && !(mn < v)) mn = v;
+}
+__device__ __forceinline__ void nan_max_step(float &mx, float v) {
+    if (v == v && !(mx > v)) mx = v;
+}
 template <typename Fetch>
 __device__ __forceinline__ float focal_reduce(const Fetch &fetch, const MaskBits &mask, int kh, int kw, int stat) {
     if (stat == XRS_STAT_MEAN || stat == XRS_STAT_VAR || stat == XRS_STAT_STD) {
@@ -339,10 +348,8 @@ __device__ __forceinline__ float focal_reduce(const Fetch &fetch, const MaskBits
             for (int kx = 0; kx < kw; ++kx)
                 if (mask.m[ky * kw + kx]) {
                     const float v = fetch(ky, kx);
-                    if (v == v) {
-                        if (!(mn < v)) mn = v;
-                        if (!(mx > v)) mx = v;
-                    }
+                    nan_min_step(mn, v);
+                    nan_max_step(mx, v);
                 }
         return stat == XRS_STAT_MIN ? mn : stat == XRS_STAT_MAX ? mx : mx - mn;
     }
@@ -472,10 +479,9 @@ focal_stat_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
             for (int r = 0; r < 4; ++r)
 #pragma unroll
                 for (int c = 0; c < 4; ++c) mn[r][c] = mx[r][c] = nan_of<float>();
-            // fminf / fmaxf return the non-NaN operand: exactly the NaN-skipping min / max
             focal_sweep(tile32, mask, g, tx, ty, [&](int r, int c, const FocalCell &q) {
-                mn[r][c] = fminf(mn[r][c], q.v);
-                mx[r][c] = fmaxf(mx[r][c], q.v);
+                nan_min_step(mn[r][c], q.v);
+                nan_max_step(mx[r][c], q.v);
             });
 #pragma unroll
             for (int r = 0; r < 4; ++r)
@@ -574,8 +580,8 @@ focal_stats_multi_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_
             focal_sweep(tile32, mask, g, tx, ty, [&](int r, int c, const FocalCell &q) {
                 const double d = q.d - mean[r][c];
                 ssd[r][c] += q.ok ? d * d : 0.0;
-                mn[r][c] = fminf(mn[r][c], q.v);
-                mx[r][c] = fmaxf(mx[r][c], q.v);
+                nan_min_step(mn[r][c], q.v);
+                nan_max_step(mx[r][c], q.v);
             });
             if (planes.p[XRS_STAT_MIN]) store_tile16(planes.p[XRS_STAT_MIN], out_pitch_elems, g.H, g.W, yo, xo, mn);
             if (planes.p[XRS_STAT_MAX]) store_tile16(planes.p[XRS_STAT_MAX], out_pitch_elems, g.H, g.W, yo, xo, mx);
@@ -768,6 +774,7 @@ int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
         const size_t smem = (size_t)nbox * g.box_h * g.sw * 4 + 16;
         if (smem <= 227 * 1024) {
             const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
+            int64_t grid = 0;
             // resident CTAs only (registers differ a lot between the statistics): the tile loop is persistent
 #define XRS_FS(ST)                                                                                              \
     case ST: {                                                                                                  \
@@ -776,7 +783,7 @@ int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
         int per_sm = 0;                                                                                         \
         XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, focal_stat_kernel<ST>, 256, smem));    \
         per_sm = per_sm < 1 ? 1 : (per_sm > 3 ? 3 : per_sm);                                                    \
-        int64_t grid = (int64_t)sms * per_sm;                                                                   \
+        grid = (int64_t)sms * per_sm;                                                                           \
         if (grid > n_tiles) grid = n_tiles;                                                                     \
         focal_stat_kernel<ST><<<(unsigned)grid, 256, smem, (cudaStream_t)s>>>(tmap, mask, out, out_pitch / 4, g); \
         break;                                                                                                  \
@@ -787,6 +794,7 @@ int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
             }
 #undef XRS_FS
             XRS_CUDA(cudaGetLastError());
+            last_launch_info() = {7, (int)grid, 256, (int)smem};
             return XRS_OK;
         }
     }
@@ -794,6 +802,7 @@ int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
     if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
     focal_stat_direct_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)s>>>(in, in_pitch / 4, mask, out, out_pitch / 4,
                                                                          H, W, kh, kw, stat);
+    last_launch_info() = {8, (int)grid, 256, 0};
     XRS_CUDA(cudaGetLastError());
     return XRS_OK;
 }
