@@ -271,8 +271,8 @@ int xrs_host_free(void *ptr);
 /* test / profiling hooks: which kernel the last launch on this thread chose -- 0 cp.async strip
  * kernel, 1 TMA strip kernel, 2 direct-ingest TMA kernel, 3 running-box kernel (uniform convolve_2d, focal.apply
  * mean over an all-ones window), 4 generic tiled convolve, 5 bounds-checked convolve fallback, 6 fused focal
- * statistics, 7 tiled single focal statistic, 8 bounds-checked focal statistic fallback -- and with how many
- * CTAs */
+ * statistics, 7 tiled single focal statistic, 8 bounds-checked focal statistic fallback, 9 zonal group-by
+ * (xrs_zonal_hash_accumulate / _run / _second_pass) -- and with how many CTAs */
 int xrs_debug_last_used_tma(void);
 int xrs_debug_last_grid(void);
 /* host-only test hook: the row-segment height the persistent kernels pick for a raster of H rows cut into

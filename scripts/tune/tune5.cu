@@ -183,7 +183,7 @@ float run(const typename Op::in_t *in, typename Op::out_t *const *outp, int64_t 
         CUtensorMap tmap;
         const int64_t pitch = W * sizeof(T);
         if (shift) W -= 4;
-        if (!make_tensor_map_2d(&tmap, in + shift, pitch, H, W, sizeof(T), kSubW, ROWS)) return -3.f;
+        if (!make_tensor_map_2d(&tmap, in + shift, pitch, H, W, dtype_of<T>(), kSubW, ROWS)) return -3.f;
         OutPtrs<Op> outs;
         for (int k = 0; k < Op::kOutputs; ++k) outs.p[k] = outp[k];
         outs.pitch_elems = pitch / sizeof(T);
@@ -197,7 +197,7 @@ float run(const typename Op::in_t *in, typename Op::out_t *const *outp, int64_t 
         int occ = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);
         if (occ < CTAS) return -1.f;
-        return time_it([&] { launch_tma<Op, ROWS, STAGES, WARPS, CTAS, T, PAD, BULK>(tmap, prm, outs, H, W, 0, 1); });
+        return time_it([&] { launch_tma<Op, ROWS, STAGES, WARPS, CTAS, T, PAD, BULK>(tmap, prm, outs, H, W, 0, kStripTma); });
     }
 }
 

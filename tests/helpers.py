@@ -1,5 +1,78 @@
-"""Shared test helpers: tolerances of the parity gate (SURVEY.md section 8d) and input makers."""
+"""Shared test helpers: tolerances of the parity gate (SURVEY.md section 8d), input makers, and the harness of
+the tests that call the C entry points on the GPU directly."""
+import ctypes
+
 import numpy as np
+
+# what xrs_debug_last_used_tma reports (LaunchKind in csrc/common.cuh)
+(K_STRIP_CPASYNC, K_STRIP_TMA, K_INGEST, K_BOX, K_CONV_TILED, K_CONV_DIRECT, K_FUSED, K_STAT_TILED, K_STAT_DIRECT,
+ K_ZONAL) = range(10)
+
+SENTINEL = 0x5A
+
+
+def gpu_lib():
+    """The loaded library module (xrspatial_b200._lib); fails when no CUDA device is present."""
+    import torch
+    import xrspatial_b200
+    assert torch.cuda.is_available(), "these tests need a CUDA device"
+    return xrspatial_b200._lib
+
+
+def stream():
+    import torch
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def last_kind(lib):
+    return lib.lib().xrs_debug_last_used_tma()
+
+
+def raster(H, W, seed, nan_frac=0.01):
+    """A float32 random-walk surface around 500 with `nan_frac` of its cells NaN."""
+    rng = np.random.default_rng(seed)
+    z = rng.standard_normal((H, W)).cumsum(0).cumsum(1) * 3.0 + 500.0
+    z[rng.random((H, W)) < nan_frac] = np.nan
+    return z.astype(np.float32)
+
+
+def in_buffer(z, pad_cols=0, rows_above=0, rows_below=0, shift=0):
+    """z on the device inside a larger buffer: `pad_cols` extra cells per row (pitch), `rows_above` /
+    `rows_below` extra rows of other data (a row-offset view), `shift` cells past the 16-byte aligned start
+    (shift=1: base and pitch not 16-byte aligned, so no TMA).  The extra cells hold large finite values, so a
+    kernel that reads them gives a visibly wrong answer.  Returns (tensor, pointer, pitch in bytes); keep the
+    tensor referenced while kernels read it."""
+    import torch
+    H, W = z.shape
+    big = np.full((H + rows_above + rows_below, W + pad_cols + shift), 9.0e3, dtype=z.dtype)
+    big[rows_above:rows_above + H, shift:shift + W] = z
+    t = torch.from_numpy(big).cuda()
+    isz = t.element_size()
+    return t, t.data_ptr() + (rows_above * t.stride(0) + shift) * isz, t.stride(0) * isz
+
+
+class Pitched(object):
+    """An output rectangle of H x W cells of `itemsize` bytes inside a sentinel-filled buffer: one row above and
+    below, 4 cells left and 8 right, so the pitch stays a multiple of 16 bytes."""
+
+    def __init__(self, H, W, itemsize=4):
+        import torch
+        self.H, self.W, self.isz = H, W, itemsize
+        self.wp = W + 12
+        self.buf = torch.full(((H + 2) * self.wp * itemsize,), SENTINEL, dtype=torch.uint8, device="cuda")
+        self.ptr = self.buf.data_ptr() + (self.wp + 4) * itemsize
+        self.pitch = self.wp * itemsize
+
+    def inside(self, what):
+        """The bytes of the H x W rectangle, as an (H, W * itemsize) uint8 array, after checking that no byte
+        outside it changed."""
+        b = self.buf.cpu().numpy().reshape(self.H + 2, self.pitch)
+        lo, hi = 4 * self.isz, (4 + self.W) * self.isz
+        ins = b[1:1 + self.H, lo:hi].copy()
+        b[1:1 + self.H, lo:hi] = SENTINEL
+        bad = int((b != SENTINEL).sum())
+        assert bad == 0, "%s: %d bytes outside the raster were written" % (what, bad)
+        return ins
 
 
 def assert_same_nan(a, b, what=""):

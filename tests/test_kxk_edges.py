@@ -16,85 +16,39 @@ import numpy as np
 import pytest
 
 import oracle as o
-from helpers import box_magnitude_fields, box_plant, box_planted_values, box_window_errors
+from helpers import (K_BOX, K_CONV_DIRECT, K_CONV_TILED, K_FUSED, K_STAT_DIRECT, K_STAT_TILED, K_STRIP_CPASYNC,
+                     K_STRIP_TMA, Pitched, box_magnitude_fields, box_plant, box_planted_values, box_window_errors,
+                     gpu_lib, in_buffer, last_kind, raster, stream)
 
 pytestmark = pytest.mark.gpu
 
 torch = pytest.importorskip("torch")
 
-SENTINEL = 0x5A
 STATS = {"mean": 0, "sum": 1, "min": 2, "max": 3, "std": 4, "range": 5, "var": 6}
 EXACT_STATS = ("mean", "sum", "min", "max", "range")
-# launch codes of xrs_debug_last_used_tma
-K_STRIP_CPASYNC, K_STRIP_TMA, K_BOX, K_CONV_TILED, K_CONV_DIRECT, K_FUSED, K_STAT_TILED, K_STAT_DIRECT = \
-    0, 1, 3, 4, 5, 6, 7, 8
 WIDTHS = [4, 124, 128, 132, 252, 256, 260, 2044, 2052]
 
 
 @pytest.fixture(scope="module")
 def lib():
-    import xrspatial_b200
-    assert torch.cuda.is_available(), "these tests need a CUDA device"
-    return xrspatial_b200._lib
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return gpu_lib()
 
 
 def _heights(kh):
     return sorted({h for h in (1, 2, kh - 1, kh, kh + 1, 63, 64, 65, 129) if h >= 1})
 
 
-def _raster(H, W, seed, nan_frac=0.01):
-    rng = np.random.default_rng(seed)
-    z = rng.standard_normal((H, W)).cumsum(0).cumsum(1) * 3.0 + 500.0
-    z[rng.random((H, W)) < nan_frac] = np.nan
-    return z.astype(np.float32)
-
-
-def _in_buffer(z, pad_cols=0, rows_above=0, rows_below=0, shift=0):
-    """z on the device inside a larger buffer: `pad_cols` extra cells per row (pitch), `rows_above` /
-    `rows_below` extra rows (a row-offset view), `shift` cells past the 16-byte aligned start (no TMA: the
-    bounds-checked kernels).  The extra cells hold a large finite value."""
-    H, W = z.shape
-    big = np.full((H + rows_above + rows_below, W + pad_cols + shift), 9.0e3, dtype=np.float32)
-    big[rows_above:rows_above + H, shift:shift + W] = z
-    t = torch.from_numpy(big).cuda()
-    return t, t.data_ptr() + (rows_above * t.stride(0) + shift) * 4, t.stride(0) * 4
-
-
-class Pitched(object):
-    """An H x W float32 output inside a sentinel-filled buffer: one row above and below, 4 cells left and 8
-    right (pitch a multiple of 16 bytes)."""
-
-    def __init__(self, H, W):
-        self.H, self.W = H, W
-        self.wp = W + 12
-        self.buf = torch.full(((H + 2) * self.wp * 4,), SENTINEL, dtype=torch.uint8, device="cuda")
-        self.ptr = self.buf.data_ptr() + (self.wp + 4) * 4
-        self.pitch = self.wp * 4
-
-    def inside(self, what):
-        b = self.buf.cpu().numpy().reshape(self.H + 2, self.pitch)
-        ins = b[1:1 + self.H, 16:16 + 4 * self.W].copy()
-        b[1:1 + self.H, 16:16 + 4 * self.W] = SENTINEL
-        bad = int((b != SENTINEL).sum())
-        assert bad == 0, "%s: %d bytes outside the raster were written" % (what, bad)
-        return ins.view(np.float32).reshape(self.H, self.W)
-
-
 def _launch(lib, call, z, view, kind, what):
     """Run `call(in_ptr, in_pitch, out_ptr, out_pitch)` on z placed as `view`; check the kernel and the
     untouched border; return the float32 result."""
     H, W = z.shape
-    t, ptr, pitch = _in_buffer(z, **view)
+    t, ptr, pitch = in_buffer(z, **view)
     out = Pitched(H, W)
     call(ptr, pitch, out.ptr, out.pitch)
     torch.cuda.synchronize()
-    got_kind = lib.lib().xrs_debug_last_used_tma()
+    got_kind = last_kind(lib)
     assert got_kind == kind, "%s: kernel %d ran, expected %d" % (what, got_kind, kind)
-    return out.inside(what)
+    return out.inside(what).view(np.float32)
 
 
 def _bits_equal(a, b, what):
@@ -116,7 +70,7 @@ def _conv_call(lib, k):
     kk = np.ascontiguousarray(k, dtype=np.float64)
 
     def call(i, ip, out, op, H, W):
-        lib.call("xrs_convolve2d_f32", i, ip, out, op, H, W, kk.ctypes.data, kh, kw, _stream())
+        lib.call("xrs_convolve2d_f32", i, ip, out, op, H, W, kk.ctypes.data, kh, kw, stream())
     return call
 
 
@@ -159,7 +113,7 @@ def test_convolve_heights(lib, kh, kw):
     k = _mixed(kh, kw, kh * 100 + kw)
     for H in _heights(kh):
         for W in (132, 260):
-            _check_conv(lib, _raster(H, W, H * 7 + W + kh), k, {}, "%dx%d on %dx%d" % (kh, kw, H, W),
+            _check_conv(lib, raster(H, W, H * 7 + W + kh), k, {}, "%dx%d on %dx%d" % (kh, kw, H, W),
                         oracle_too=kh * kw * H * W <= 3e7)
 
 
@@ -169,7 +123,7 @@ def test_convolve_widths(lib, kh, kw):
     k = _mixed(kh, kw, kh * 10 + kw)
     for W in WIDTHS:
         H = 65
-        _check_conv(lib, _raster(H, W, W + kh), k, {}, "%dx%d on %dx%d" % (kh, kw, H, W),
+        _check_conv(lib, raster(H, W, W + kh), k, {}, "%dx%d on %dx%d" % (kh, kw, H, W),
                     oracle_too=kh * kw * H * W <= 3e7)
 
 
@@ -178,7 +132,7 @@ def test_convolve_zero_taps(lib, k):
     """Circle weights: a NaN under a zero tap still makes the window NaN (0 * NaN is NaN in the reference)."""
     w = _circle(k) * 0.01
     w[k // 2, k // 2] = -0.5
-    z = _raster(129, 260, k, nan_frac=0.003)
+    z = raster(129, 260, k, nan_frac=0.003)
     _check_conv(lib, z, w, {}, "circle %d" % k)
 
 
@@ -189,14 +143,14 @@ def test_convolve_pitched_and_offset_views(lib, kh, kw):
     k = _mixed(kh, kw, kh + kw)
     for W in (252, 2052):
         pad = (-(W * 4) % 128 + 16) // 4
-        _check_conv(lib, _raster(67, W, W), k, {"pad_cols": pad}, "%dx%d pitch +16 B, W %d" % (kh, kw, W))
-        _check_conv(lib, _raster(41, W, W + 1), k, {"rows_above": 3, "rows_below": 2},
+        _check_conv(lib, raster(67, W, W), k, {"pad_cols": pad}, "%dx%d pitch +16 B, W %d" % (kh, kw, W))
+        _check_conv(lib, raster(41, W, W + 1), k, {"rows_above": 3, "rows_below": 2},
                     "%dx%d row-offset view, W %d" % (kh, kw, W))
 
 
 def test_convolve_kernel_larger_than_raster(lib):
     for kh, kw, H, W in ((25, 25, 7, 12), (49, 49, 20, 4), (63, 1, 30, 8), (1, 31, 3, 16)):
-        _check_conv(lib, _raster(H, W, kh + H), _mixed(kh, kw, W), {}, "%dx%d on %dx%d" % (kh, kw, H, W))
+        _check_conv(lib, raster(H, W, kh + H), _mixed(kh, kw, W), {}, "%dx%d on %dx%d" % (kh, kw, H, W))
 
 
 # ----------------------------------------------------------------------------------------- focal statistics
@@ -205,7 +159,7 @@ def _stat_call(lib, k, stat):
     kk = np.ascontiguousarray(k, dtype=np.float64)
 
     def call(i, ip, out, op, H, W):
-        lib.call("xrs_focal_stat_f32", i, ip, out, op, H, W, kk.ctypes.data, kh, kw, STATS[stat], _stream())
+        lib.call("xrs_focal_stat_f32", i, ip, out, op, H, W, kk.ctypes.data, kh, kw, STATS[stat], stream())
     return call
 
 
@@ -276,7 +230,7 @@ def _masks():
 def test_focal_stats_masks(lib, name):
     k = _masks()[name]
     for H, W in ((129, 260), (65, 132), (k.shape[0], 128), (2, 252)):
-        _check_stats(lib, _raster(H, W, H + W + k.size), k, {}, "%s on %dx%d" % (name, H, W))
+        _check_stats(lib, raster(H, W, H + W + k.size), k, {}, "%s on %dx%d" % (name, H, W))
         _check_stats(lib, _signed_zero_raster(H, W, H * W), k, {}, "%s signed zeros on %dx%d" % (name, H, W))
 
 
@@ -323,13 +277,13 @@ def test_fused_focal_stats_bit_exact(lib, name):
     ids = np.array(list(STATS.values()), dtype=np.int32)
     for H, W in ((129, 260), (3, 132)):
         z = _signed_zero_raster(H, W, H + W + 1)
-        t, ptr, pitch = _in_buffer(z)
+        t, ptr, pitch = in_buffer(z)
         plane = (H * W * 4 + 15) // 16 * 16
         out = torch.full((len(ids) * plane // 4,), -1.0, dtype=torch.float32, device="cuda")
         lib.call("xrs_focal_stats_multi_f32", ptr, pitch, out.data_ptr(), W * 4, plane, H, W, kk.ctypes.data,
-                 k.shape[0], k.shape[1], ids.ctypes.data, len(ids), _stream())
+                 k.shape[0], k.shape[1], ids.ctypes.data, len(ids), stream())
         torch.cuda.synchronize()
-        assert lib.lib().xrs_debug_last_used_tma() == K_FUSED
+        assert last_kind(lib) == K_FUSED
         res = out.cpu().numpy()
         for i, (stat, sid) in enumerate(STATS.items()):
             got = res[i * plane // 4:i * plane // 4 + H * W].reshape(H, W)
@@ -348,13 +302,13 @@ def test_ragged_width_falls_back_per_plane(lib):
     k = _circle(5)
     kk = np.ascontiguousarray(k, dtype=np.float64)
     ids = np.array([0, 2, 3], dtype=np.int32)
-    t, ptr, pitch = _in_buffer(z)
+    t, ptr, pitch = in_buffer(z)
     plane = (H * W * 4 + 15) // 16 * 16
     out = torch.full((3 * plane // 4,), -1.0, dtype=torch.float32, device="cuda")
     lib.call("xrs_focal_stats_multi_f32", ptr, pitch, out.data_ptr(), W * 4, plane, H, W, kk.ctypes.data, 5, 5,
-             ids.ctypes.data, 3, _stream())
+             ids.ctypes.data, 3, stream())
     torch.cuda.synchronize()
-    assert lib.lib().xrs_debug_last_used_tma() == K_STAT_DIRECT
+    assert last_kind(lib) == K_STAT_DIRECT
     res = out.cpu().numpy()
     for i, stat in enumerate(("mean", "min", "max")):
         got = res[i * plane // 4:i * plane // 4 + H * W].reshape(H, W)

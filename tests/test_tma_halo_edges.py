@@ -5,10 +5,10 @@ cells) in boxes of 208 cells; cells left of column 0 and right of W arrive as Na
 NaN from their coordinates (integer maps).  These tests compare the TMA kernels bit for bit with the cp.async
 kernel, which fills its ring cell by cell with bounds checks, at widths around the halo, box and tile edges, on
 pitched and row-offset inputs, and for every direct-ingest dtype.  Runs on an H100 (`-m gpu`)."""
-import ctypes
-
 import numpy as np
 import pytest
+
+from helpers import K_INGEST, K_STRIP_CPASYNC, K_STRIP_TMA, gpu_lib, in_buffer, last_kind, raster, stream
 
 pytestmark = pytest.mark.gpu
 
@@ -21,61 +21,36 @@ HEIGHTS = [1, 2, 3, 5, 67]
 
 @pytest.fixture(scope="module")
 def lib():
-    import xrspatial_b200
-    assert torch.cuda.is_available(), "these tests need a CUDA device"
-    return xrspatial_b200._lib
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _raster(H, W, seed):
-    rng = np.random.default_rng(seed)
-    z = rng.standard_normal((H, W)).cumsum(0).cumsum(1) * 3.0 + 500.0
-    z[rng.random((H, W)) < 0.01] = np.nan
-    return z.astype(np.float32)
-
-
-def _in_buffer(z, pad_cols=0, rows_above=0, rows_below=0, shift=0):
-    """z on the device inside a larger buffer: `pad_cols` extra cells per row (pitch), `rows_above` /
-    `rows_below` extra rows of other data (a row-offset view), `shift` cells past the 16-byte aligned start.
-    The extra cells hold large finite values, so a kernel that reads them gives a visibly wrong answer."""
-    H, W = z.shape
-    big = np.full((H + rows_above + rows_below, W + pad_cols + shift), 9.0e3, dtype=z.dtype)
-    big[rows_above:rows_above + H, shift:shift + W] = z
-    t = torch.from_numpy(big).cuda()
-    isz = t.element_size()
-    return t, t.data_ptr() + (rows_above * t.stride(0) + shift) * isz, t.stride(0) * isz
+    return gpu_lib()
 
 
 def _run(lib, fn, in_ptr, in_pitch, H, W, kind):
     out = torch.full((H, W), -1.0, dtype=torch.float32, device="cuda")
     fn(in_ptr, in_pitch, out.data_ptr(), W * 4)
     torch.cuda.synchronize()
-    assert lib.lib().xrs_debug_last_used_tma() == kind
+    assert last_kind(lib) == kind
     return out.cpu().numpy().view(np.uint32)
 
 
 def _ops(lib, H, W):
     ex = np.array([np.nan], dtype=np.float64)
     return {
-        "slope": lambda i, ip, o, op: lib.call("xrs_slope_f32", i, ip, o, op, H, W, 30.0, 30.0, _stream()),
-        "hillshade": lambda i, ip, o, op: lib.call("xrs_hillshade_f32", i, ip, o, op, H, W, 225.0, 25.0, _stream()),
+        "slope": lambda i, ip, o, op: lib.call("xrs_slope_f32", i, ip, o, op, H, W, 30.0, 30.0, stream()),
+        "hillshade": lambda i, ip, o, op: lib.call("xrs_hillshade_f32", i, ip, o, op, H, W, 225.0, 25.0, stream()),
         "focal.mean": lambda i, ip, o, op: lib.call("xrs_focal_mean_f32", i, ip, o, op, H, W,
-                                                    ex.ctypes.data, 1, _stream()),
+                                                    ex.ctypes.data, 1, stream()),
         "suite": lambda i, ip, o, op: lib.call("xrs_surface_suite_f32", i, ip, None, None, None, o, op, H, W,
-                                               30.0, 30.0, 225.0, 25.0, _stream()),
+                                               30.0, 30.0, 225.0, 25.0, stream()),
     }
 
 
 def _compare(lib, H, W, tma_view, seed):
-    z = _raster(H, W, seed)
-    ta, pa, ia = _in_buffer(z, **tma_view)    # the tensors stay referenced while the kernels read them
-    tm, pm, im = _in_buffer(z, shift=1)       # base not 16-byte aligned: the cp.async kernel
+    z = raster(H, W, seed)
+    ta, pa, ia = in_buffer(z, **tma_view)    # the tensors stay referenced while the kernels read them
+    tm, pm, im = in_buffer(z, shift=1)       # base not 16-byte aligned: the cp.async kernel
     for name, fn in _ops(lib, H, W).items():
-        got = _run(lib, fn, pa, ia, H, W, 1)
-        ref = _run(lib, fn, pm, im, H, W, 0)
+        got = _run(lib, fn, pa, ia, H, W, K_STRIP_TMA)
+        ref = _run(lib, fn, pm, im, H, W, K_STRIP_CPASYNC)
         np.testing.assert_array_equal(got, ref, err_msg="%s %dx%d %s: cells differ" % (name, H, W, tma_view))
 
 
@@ -104,7 +79,7 @@ def test_row_offset_view(lib, W):
 def test_direct_ingest_edges(lib, dtype, code, H, W):
     """int16 / uint16 / int32 / float64 read directly at the left and right raster edges vs the float32 kernels
     on the cast raster (cp.async path); slope with rectangular cells and hillshade."""
-    z = _raster(H, W, 7 * H + W + code)
+    z = raster(H, W, 7 * H + W + code)
     if np.issubdtype(dtype, np.integer):
         lo = 0 if dtype == np.uint16 else -30000
         z = np.nan_to_num(np.round(z), nan=-7.0).clip(lo, 30000)
@@ -113,17 +88,17 @@ def test_direct_ingest_edges(lib, dtype, code, H, W):
     buf = np.zeros((H, wq), dtype=dtype)
     buf[:, :W] = zs
     ts = torch.from_numpy(buf).cuda()
-    tm, pm, im = _in_buffer(zs.astype(np.float32), shift=1)
+    tm, pm, im = in_buffer(zs.astype(np.float32), shift=1)
     cells = np.array([10.0, 25.5])
     sun = np.array([225.0, 25.0])
     cases = [
-        ("slope", 0, cells, lambda o, op: lib.call("xrs_slope_f32", pm, im, o, op, H, W, 10.0, 25.5, _stream())),
+        ("slope", 0, cells, lambda o, op: lib.call("xrs_slope_f32", pm, im, o, op, H, W, 10.0, 25.5, stream())),
         ("hillshade", 3, sun, lambda o, op: lib.call("xrs_hillshade_f32", pm, im, o, op, H, W, 225.0, 25.0,
-                                                     _stream())),
+                                                     stream())),
     ]
     for name, op_code, par, ref_fn in cases:
         got = _run(lib, lambda i, ip, o, op: lib.call("xrs_surface_typed", op_code, i, code, ip, o, op, H, W,
-                                                      par.ctypes.data, _stream()),
-                   ts.data_ptr(), wq * zs.itemsize, H, W, 2)
-        ref = _run(lib, lambda i, ip, o, op: ref_fn(o, op), 0, 0, H, W, 0)
+                                                      par.ctypes.data, stream()),
+                   ts.data_ptr(), wq * zs.itemsize, H, W, K_INGEST)
+        ref = _run(lib, lambda i, ip, o, op: ref_fn(o, op), 0, 0, H, W, K_STRIP_CPASYNC)
         np.testing.assert_array_equal(got, ref, err_msg="%s %s %dx%d: cells differ" % (name, zs.dtype, H, W))

@@ -487,7 +487,7 @@ static int launch_box_stream2(const float *in, int64_t in_pitch, float *out, int
                               int kh, double w, cudaStream_t s) {
     using S = B2Shape<RX, NW>;
     CUtensorMap tmap;
-    if (!make_tensor_map_2d(&tmap, in, in_pitch, H, W, 4, S::kBoxW, kB2Rows)) return kBoxNotTaken;
+    if (!make_tensor_map_2d(&tmap, in, in_pitch, H, W, XRS_F32, S::kBoxW, kB2Rows)) return kBoxNotTaken;
     B2Geom g;
     g.H = H; g.W = W; g.kh = kh; g.ry = kh / 2; g.w = w;
     g.n_cells = (double)(kh * (2 * RX + 1));
@@ -499,30 +499,22 @@ static int launch_box_stream2(const float *in, int64_t in_pitch, float *out, int
     if (max_ctas < 1) max_ctas = 1;
     if (want < 1) want = 1;
     const size_t stage_bytes = (size_t)2 * S::kHalfBytes;
-    // shared memory of an SM: 228 KB, 1 KB of it reserved per resident CTA
-    const size_t cap = ((size_t)228 * 1024 - (size_t)max_ctas * 1024) / max_ctas - 256;
+    const size_t cap = (kSmemPerSm - (size_t)max_ctas * kSmemReservedPerCta) / max_ctas - 256;
     if (stages < 2) stages = 2;
     while (stages > 2 && (size_t)stages * stage_bytes + (size_t)2 * stages * sizeof(uint64_t) > cap) --stages;
     g.stages = stages;
     const size_t smem = (size_t)stages * stage_bytes + (size_t)2 * stages * sizeof(uint64_t);
     auto kern = box_stream2_kernel<RX, NW, MODE>;
-    XRS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, (NW + 1) * 32, smem));
-    if (per_sm < 1) per_sm = 1;
-    if (per_sm > max_ctas) per_sm = max_ctas;
-    const int64_t resident = (int64_t)sm_count() * per_sm;
+    int64_t resident;
+    if (const int rc = resident_ctas(kern, (NW + 1) * 32, smem, max_ctas, &resident)) return rc;
     // segments: tall enough that the kh - 1 lead-in rows stay a small overhead, (rows + kh - 1) a
     // multiple of 4 so that only the raster's last segment ends in a partial batch
     const int64_t seg_rows = pick_seg_rows(H, g.n_tiles, resident, 12 * (int64_t)kh, kh - 1, kB2Rows, want);
     g.seg_rows = (int)seg_rows;
     g.n_segs = (int)((H + seg_rows - 1) / seg_rows);
     const int64_t n_tasks = (int64_t)g.n_tiles * g.n_segs;
-    const int64_t grid = resident < n_tasks ? resident : n_tasks;
-    kern<<<(unsigned)grid, (NW + 1) * 32, smem, s>>>(tmap, in, in_pitch / 4, out, out_pitch / 4, g);
-    last_launch_info() = {3, (int)grid, (NW + 1) * 32, (int)smem};
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    return launch(kern, resident < n_tasks ? resident : n_tasks, (NW + 1) * 32, smem, s, kRunningBox, tmap, in,
+                  in_pitch / 4, out, out_pitch / 4, g);
 }
 
 // true when the streaming box kernel took the job (*rc = its status)

@@ -2,9 +2,12 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+
+#include <type_traits>
 
 #include "../../include/xrs_b200.h"
 
@@ -14,10 +17,22 @@ namespace xrs {
 void set_error(const char *fmt, ...);
 int cuda_fail(cudaError_t e, const char *what);
 
+// Which kernel a launch ran (xrs_debug_last_used_tma reports it; the codes are listed in xrs_b200.h).
+enum LaunchKind : int {
+    kStripCpAsync = 0,  // 3x3 strip kernel, per-warp cp.async ring
+    kStripTma = 1,      // 3x3 strip kernel, CTA-wide TMA ring
+    kIngestTma = 2,     // 3x3 TMA strip kernel reading int16 / uint16 / int32 / float64 cells
+    kRunningBox = 3,    // running-box convolve_2d / focal.apply mean
+    kConvTiled = 4,     // tiled k x k convolve
+    kConvDirect = 5,    // bounds-checked convolve
+    kFocalFused = 6,    // every requested focal statistic in one pass
+    kFocalTiled = 7,    // tiled single focal statistic
+    kFocalDirect = 8,   // bounds-checked single focal statistic
+    kZonalHash = 9,     // zonal group-by
+};
+
 struct LaunchInfo {  // for tests / profiling: what the last launch on this thread chose
-    int used_tma;    // 0 cp.async strip kernel, 1 TMA strip kernel, 2 direct-ingest, 3 running-box kernel,
-                     // 4 generic tiled convolve, 5 bounds-checked convolve fallback, 6 fused focal statistics,
-                     // 7 tiled focal statistic, 8 bounds-checked focal statistic fallback
+    int kind;        // a LaunchKind
     int grid, block, smem_bytes;
 };
 LaunchInfo &last_launch_info();
@@ -39,12 +54,45 @@ LaunchInfo &last_launch_info();
 // cached per-device properties
 int sm_count(int device = -1);
 
-// Encodes a 2-D tiled tensor map over a row-major (H, W) raster of `elem_bytes` elements
-// with out-of-bounds fill = NaN (the raster-edge semantics of the reference's
-// `boundary=np.nan` overlap, slope.py:94-97).  Returns false if TMA cannot describe it
-// (base/pitch not 16-byte aligned, ...); callers then use the direct-load kernels.
-bool make_tensor_map_2d(CUtensorMap *map, const void *base, int64_t pitch_bytes, int64_t H,
-                        int64_t W, int elem_bytes, int box_w, int box_h);
+// Shared memory of an H100 SM: 228 KB, at most 227 KB of it for one CTA, 1 KB reserved per resident CTA.
+constexpr size_t kSmemPerSm = 228 * 1024, kSmemPerCtaMax = 227 * 1024, kSmemReservedPerCta = 1024;
+
+// Persistent kernels: sets `kernel`'s dynamic shared-memory limit to `smem`, then *resident = the CTAs of
+// `threads` threads that fit on the device at once, between 1 and max_per_sm per SM.
+int resident_ctas(const void *kernel, int threads, size_t smem, int max_per_sm, int64_t *resident);
+template <typename... P>
+int resident_ctas(void (*kernel)(P...), int threads, size_t smem, int max_per_sm, int64_t *resident) {
+    return resident_ctas(reinterpret_cast<const void *>(kernel), threads, smem, max_per_sm, resident);
+}
+
+// Records the launch in last_launch_info(), launches `kernel` and reports a launch error.
+template <typename... P, typename... A>
+int launch(void (*kernel)(P...), int64_t grid, int threads, size_t smem, cudaStream_t stream, LaunchKind kind,
+           const A &...args) {
+    last_launch_info() = {kind, (int)grid, threads, (int)smem};
+    kernel<<<(unsigned)grid, threads, smem, stream>>>(args...);
+    XRS_CUDA(cudaGetLastError());
+    return XRS_OK;
+}
+
+// Encodes a 2-D tiled tensor map over a row-major (H, W) raster of `dtype` cells (float32, float64, int32,
+// int16 or uint16).  Float cells beyond the raster read as NaN (the raster-edge semantics of the reference's
+// `boundary=np.nan` overlap, slope.py:94-97); integer cells read as 0, and their kernels substitute NaN from
+// the cell coordinates.  Returns false if TMA cannot describe the raster (base / pitch not 16-byte aligned,
+// ...); callers then use kernels that load without TMA.
+bool make_tensor_map_2d(CUtensorMap *map, const void *base, int64_t pitch_bytes, int64_t H, int64_t W,
+                        xrs_dtype dtype, int box_w, int box_h);
+
+template <typename T> constexpr xrs_dtype dtype_of() {
+    if constexpr (std::is_same_v<T, float>) return XRS_F32;
+    else if constexpr (std::is_same_v<T, double>) return XRS_F64;
+    else if constexpr (std::is_same_v<T, int>) return XRS_I32;
+    else if constexpr (std::is_same_v<T, short>) return XRS_I16;
+    else {
+        static_assert(std::is_same_v<T, unsigned short>, "no tensor-map element type");
+        return XRS_U16;
+    }
+}
 
 // ----------------------------------------------------------------------------- device PTX
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
@@ -87,12 +135,7 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
         "l"(map), "r"(smem_u32(bar)), "r"(x), "r"(y)
         : "memory");
 }
-// same, with an L2 eviction-priority hint (a policy from l2_policy_evict_first / l2_policy_evict_last)
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
+// same, with an L2 eviction-priority hint (a policy from l2_policy_evict_last)
 __device__ __forceinline__ void tma_load_2d_hint(void *dst, const CUtensorMap *map, uint64_t *bar, int x, int y,
                                                  uint64_t policy) {
     asm volatile(

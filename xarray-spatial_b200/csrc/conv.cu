@@ -38,7 +38,29 @@ struct TileGeom {
     int sh;        // shared tile height = kTileH + kh - 1
     int tiles_x, tiles_y;
     int box_h;     // rows per TMA box (sh is loaded in ceil(sh / box_h) boxes)
+    __host__ __device__ size_t tile_cells() const { return (size_t)((sh + box_h - 1) / box_h) * box_h * sw; }
+    size_t smem_bytes() const { return tile_cells() * sizeof(float) + 16; }   // the tile, then its mbarrier
 };
+
+// The tiled kernels' shared memory: the (tile + halo) block, then one mbarrier.  Thread 0 prefetches the
+// tensor-map descriptor and initialises the barrier; every thread returns after the CTA barrier.
+struct SmemTile {
+    float *tile32;
+    uint64_t *bar;
+};
+__device__ __forceinline__ SmemTile tile_preamble(const CUtensorMap *tmap, const TileGeom &g) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    SmemTile s;
+    s.tile32 = reinterpret_cast<float *>(smem_raw);
+    s.bar = reinterpret_cast<uint64_t *>(smem_raw + g.tile_cells() * sizeof(float));
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(tmap);
+        mbar_init(s.bar, 1);
+        mbar_fence_init();
+    }
+    __syncthreads();
+    return s;
+}
 
 __device__ __forceinline__ void load_tile_tma(const CUtensorMap *tmap, float *tile32, uint64_t *bar,
                                               const TileGeom &g, int tx0, int ty0, uint32_t parity) {
@@ -66,18 +88,7 @@ template <int KW>
 __global__ void __launch_bounds__(256)
 conv2d_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ ConvWeights cw,
               float *__restrict__ out, int64_t out_pitch_elems, const TileGeom g) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const int nbox = (g.sh + g.box_h - 1) / g.box_h;
-    const size_t tile_cells = (size_t)nbox * g.box_h * g.sw;
-    float *tile32 = reinterpret_cast<float *>(smem_raw);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem_raw + tile_cells * sizeof(float));
-
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmap);
-        mbar_init(bar, 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
+    const auto [tile32, bar] = tile_preamble(&tmap, g);
 
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
     const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
@@ -207,17 +218,7 @@ conv2d_fixed_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_const
                     float *__restrict__ out, int64_t out_pitch_elems, const TileGeom g) {
     constexpr int kOff = (K / 2 + 3) / 4 * 4 - K / 2;   // column of tap 0 relative to the aligned origin
     constexpr int kVals = (kOff + K + 3 + 3) / 4 * 4;   // cells a thread needs per row and half
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const int nbox = (g.sh + g.box_h - 1) / g.box_h;
-    const size_t tile_cells = (size_t)nbox * g.box_h * g.sw;
-    float *tile32 = reinterpret_cast<float *>(smem_raw);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem_raw + tile_cells * sizeof(float));
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmap);
-        mbar_init(bar, 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
+    const auto [tile32, bar] = tile_preamble(&tmap, g);
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
     const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
     uint32_t parity = 0;
@@ -413,17 +414,7 @@ template <int STAT>
 __global__ void __launch_bounds__(256)
 focal_stat_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ MaskBits mask,
                   float *__restrict__ out, int64_t out_pitch_elems, const TileGeom g) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const int nbox = (g.sh + g.box_h - 1) / g.box_h;
-    const size_t tile_cells = (size_t)nbox * g.box_h * g.sw;
-    float *tile32 = reinterpret_cast<float *>(smem_raw);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem_raw + tile_cells * sizeof(float));
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmap);
-        mbar_init(bar, 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
+    const auto [tile32, bar] = tile_preamble(&tmap, g);
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
     const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
     uint32_t parity = 0;
@@ -524,17 +515,7 @@ __device__ __forceinline__ void store_tile16(float *plane, int64_t pitch_elems, 
 __global__ void __launch_bounds__(256, 2)
 focal_stats_multi_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ MaskBits mask,
                          const StatPlanes planes, int64_t out_pitch_elems, const TileGeom g) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const int nbox = (g.sh + g.box_h - 1) / g.box_h;
-    const size_t tile_cells = (size_t)nbox * g.box_h * g.sw;
-    float *tile32 = reinterpret_cast<float *>(smem_raw);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem_raw + tile_cells * sizeof(float));
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmap);
-        mbar_init(bar, 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
+    const auto [tile32, bar] = tile_preamble(&tmap, g);
     const bool want_b = planes.p[XRS_STAT_MIN] || planes.p[XRS_STAT_MAX] || planes.p[XRS_STAT_RANGE] ||
                         planes.p[XRS_STAT_STD] || planes.p[XRS_STAT_VAR];
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -655,7 +636,19 @@ static bool tile_geom(TileGeom &g, CUtensorMap *tmap, const float *in, int64_t i
     g.box_h = g.sh <= 64 ? g.sh : 64;  // 64 % 8 == 0 keeps the following boxes 128-byte aligned
     if (g.sw > 256) return false;
     if (W % 4 != 0 || out_pitch % 16 != 0 || (reinterpret_cast<uintptr_t>(out) & 15)) return false;
-    return make_tensor_map_2d(tmap, in, in_pitch, H, W, 4, g.sw, g.box_h);
+    return make_tensor_map_2d(tmap, in, in_pitch, H, W, XRS_F32, g.sw, g.box_h) && g.smem_bytes() <= kSmemPerCtaMax;
+}
+
+// The persistent tiled kernels: 256 threads, as many CTAs as fit (at most max_per_sm per SM), never more CTAs
+// than tiles.
+template <typename... P, typename... A>
+static int launch_tiles(void (*kern)(P...), const TileGeom &g, int max_per_sm, cudaStream_t s, LaunchKind kind,
+                        const A &...args) {
+    const size_t smem = g.smem_bytes();
+    int64_t resident;
+    if (const int rc = resident_ctas(kern, 256, smem, max_per_sm, &resident)) return rc;
+    const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
+    return launch(kern, resident < n_tiles ? resident : n_tiles, 256, smem, s, kind, args...);
 }
 
 }  // namespace xrs
@@ -689,65 +682,28 @@ int xrs_convolve2d_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
     for (int i = 0; i < kh * kw; ++i) cw.w[i] = kernel[i];
     TileGeom g;
     CUtensorMap tmap;
-    const int sms = sm_count();
     if (tile_geom(g, &tmap, in, in_pitch, out, out_pitch, H, W, kh, kw, kConvTileH)) {
-        const int nbox = (g.sh + g.box_h - 1) / g.box_h;
-        const size_t cells = (size_t)nbox * g.box_h * g.sw;
-        const size_t smem = cells * 4 + 16;
-        if (smem <= 227 * 1024) {
-            const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
-            int64_t grid = 0;
-#define XRS_CONV(KWC)                                                                                          \
-    {                                                                                                          \
-        XRS_CUDA(cudaFuncSetAttribute(conv2d_kernel<KWC>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
-                                      (int)smem));                                                             \
-        int per_sm = 0;                                                                                        \
-        XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv2d_kernel<KWC>, 256, smem));      \
-        if (per_sm < 1) per_sm = 1;                                                                            \
-        grid = (int64_t)sms * per_sm;                                                                          \
-        if (grid > n_tiles) grid = n_tiles;                                                                    \
-        conv2d_kernel<KWC><<<(unsigned)grid, 256, smem, (cudaStream_t)s>>>(tmap, cw, out, out_pitch / 4, g);  \
-    }
-#define XRS_CONVF(KC)                                                                                           \
-    {                                                                                                          \
-        XRS_CUDA(cudaFuncSetAttribute(conv2d_fixed_kernel<KC>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
-                                      (int)smem));                                                             \
-        int per_sm = 0;                                                                                        \
-        XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv2d_fixed_kernel<KC>, 256, smem)); \
-        if (per_sm < 1) per_sm = 1;                                                                            \
-        grid = (int64_t)sms * per_sm;                                                                          \
-        if (grid > n_tiles) grid = n_tiles;                                                                    \
-        conv2d_fixed_kernel<KC><<<(unsigned)grid, 256, smem, (cudaStream_t)s>>>(tmap, cw, out, out_pitch / 4, g); \
-    }
-            if (kh == kw && kw >= 5 && kw <= 13) {
-                switch (kw) {
-                    case 5: XRS_CONVF(5) break;
-                    case 7: XRS_CONVF(7) break;
-                    case 11: XRS_CONVF(11) break;
-                    case 13: XRS_CONVF(13) break;
-                    default: XRS_CONVF(9) break;
-                }
-            } else
+        auto kern = conv2d_kernel<0>;
+        if (kh == kw && kw >= 5 && kw <= 13) {
             switch (kw) {
-                case 5: XRS_CONV(5) break;
-                case 7: XRS_CONV(7) break;
-                case 9: XRS_CONV(9) break;
-                default: XRS_CONV(0) break;
+                case 5: kern = conv2d_fixed_kernel<5>; break;
+                case 7: kern = conv2d_fixed_kernel<7>; break;
+                case 11: kern = conv2d_fixed_kernel<11>; break;
+                case 13: kern = conv2d_fixed_kernel<13>; break;
+                default: kern = conv2d_fixed_kernel<9>; break;
             }
-#undef XRS_CONV
-#undef XRS_CONVF
-            XRS_CUDA(cudaGetLastError());
-            last_launch_info() = {4, (int)grid, 256, (int)smem};
-            return XRS_OK;
+        } else {
+            switch (kw) {
+                case 5: kern = conv2d_kernel<5>; break;
+                case 7: kern = conv2d_kernel<7>; break;
+                case 9: kern = conv2d_kernel<9>; break;
+            }
         }
+        return launch_tiles(kern, g, INT_MAX, (cudaStream_t)s, kConvTiled, tmap, cw, out, out_pitch / 4, g);
     }
-    int64_t grid = (H * W + 255) / 256;
-    if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
-    conv2d_direct_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)s>>>(in, in_pitch / 4, cw, out, out_pitch / 4, H, W,
-                                                                     kh, kw);
-    last_launch_info() = {5, (int)grid, 256, 0};
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    const int64_t cell_ctas = (H * W + 255) / 256, max_ctas = (int64_t)sm_count() * 8;
+    return launch(conv2d_direct_kernel, cell_ctas < max_ctas ? cell_ctas : max_ctas, 256, 0, (cudaStream_t)s,
+                  kConvDirect, in, in_pitch / 4, cw, out, out_pitch / 4, H, W, kh, kw);
 }
 
 int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
@@ -768,43 +724,22 @@ int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
     }
     TileGeom g;
     CUtensorMap tmap;
-    const int sms = sm_count();
     if (tile_geom(g, &tmap, in, in_pitch, out, out_pitch, H, W, kh, kw, kTileH)) {
-        const int nbox = (g.sh + g.box_h - 1) / g.box_h;
-        const size_t smem = (size_t)nbox * g.box_h * g.sw * 4 + 16;
-        if (smem <= 227 * 1024) {
-            const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
-            int64_t grid = 0;
-            // resident CTAs only (registers differ a lot between the statistics): the tile loop is persistent
-#define XRS_FS(ST)                                                                                              \
-    case ST: {                                                                                                  \
-        XRS_CUDA(cudaFuncSetAttribute(focal_stat_kernel<ST>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
-                                      (int)smem));                                                              \
-        int per_sm = 0;                                                                                         \
-        XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, focal_stat_kernel<ST>, 256, smem));    \
-        per_sm = per_sm < 1 ? 1 : (per_sm > 3 ? 3 : per_sm);                                                    \
-        grid = (int64_t)sms * per_sm;                                                                           \
-        if (grid > n_tiles) grid = n_tiles;                                                                     \
-        focal_stat_kernel<ST><<<(unsigned)grid, 256, smem, (cudaStream_t)s>>>(tmap, mask, out, out_pitch / 4, g); \
-        break;                                                                                                  \
-    }
-            switch (stat) {
-                XRS_FS(XRS_STAT_MEAN) XRS_FS(XRS_STAT_SUM) XRS_FS(XRS_STAT_MIN) XRS_FS(XRS_STAT_MAX)
-                XRS_FS(XRS_STAT_STD) XRS_FS(XRS_STAT_RANGE) XRS_FS(XRS_STAT_VAR)
-            }
-#undef XRS_FS
-            XRS_CUDA(cudaGetLastError());
-            last_launch_info() = {7, (int)grid, 256, (int)smem};
-            return XRS_OK;
+        auto kern = focal_stat_kernel<XRS_STAT_MEAN>;
+        switch (stat) {
+            case XRS_STAT_SUM: kern = focal_stat_kernel<XRS_STAT_SUM>; break;
+            case XRS_STAT_MIN: kern = focal_stat_kernel<XRS_STAT_MIN>; break;
+            case XRS_STAT_MAX: kern = focal_stat_kernel<XRS_STAT_MAX>; break;
+            case XRS_STAT_STD: kern = focal_stat_kernel<XRS_STAT_STD>; break;
+            case XRS_STAT_RANGE: kern = focal_stat_kernel<XRS_STAT_RANGE>; break;
+            case XRS_STAT_VAR: kern = focal_stat_kernel<XRS_STAT_VAR>; break;
         }
+        // at most 3 CTAs per SM (registers differ a lot between the statistics): the tile loop is persistent
+        return launch_tiles(kern, g, 3, (cudaStream_t)s, kFocalTiled, tmap, mask, out, out_pitch / 4, g);
     }
-    int64_t grid = (H * W + 255) / 256;
-    if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
-    focal_stat_direct_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)s>>>(in, in_pitch / 4, mask, out, out_pitch / 4,
-                                                                         H, W, kh, kw, stat);
-    last_launch_info() = {8, (int)grid, 256, 0};
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    const int64_t cell_ctas = (H * W + 255) / 256, max_ctas = (int64_t)sm_count() * 8;
+    return launch(focal_stat_direct_kernel, cell_ctas < max_ctas ? cell_ctas : max_ctas, 256, 0, (cudaStream_t)s,
+                  kFocalDirect, in, in_pitch / 4, mask, out, out_pitch / 4, H, W, kh, kw, stat);
 }
 
 int xrs_focal_stats_multi_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t plane_stride,
@@ -825,25 +760,10 @@ int xrs_focal_stats_multi_f32(const float *in, int64_t in_pitch, float *out, int
     TileGeom g;
     CUtensorMap tmap;
     if (n_stats >= 2 && tile_geom(g, &tmap, in, in_pitch, out, out_pitch, H, W, kh, kw, kTileH)) {
-        const int nbox = (g.sh + g.box_h - 1) / g.box_h;
-        const size_t smem = (size_t)nbox * g.box_h * g.sw * 4 + 16;
-        if (smem <= 227 * 1024) {
-            static thread_local MaskBits mask;
-            for (int i = 0; i < kh * kw; ++i) mask.m[i] = (kernel[i] == 1.0) ? 1 : 0;  // focal.py:323
-            XRS_CUDA(cudaFuncSetAttribute(focal_stats_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)smem));
-            int per_sm = 0;
-            XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, focal_stats_multi_kernel, 256, smem));
-            if (per_sm < 1) per_sm = 1;
-            if (per_sm > 3) per_sm = 3;
-            int64_t grid = (int64_t)sm_count() * per_sm;
-            const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
-            if (grid > n_tiles) grid = n_tiles;
-            focal_stats_multi_kernel<<<(unsigned)grid, 256, smem, (cudaStream_t)s>>>(tmap, mask, planes, out_pitch / 4, g);
-            XRS_CUDA(cudaGetLastError());
-            last_launch_info() = {6, (int)grid, 256, (int)smem};
-            return XRS_OK;
-        }
+        static thread_local MaskBits mask;
+        for (int i = 0; i < kh * kw; ++i) mask.m[i] = (kernel[i] == 1.0) ? 1 : 0;  // focal.py:323
+        return launch_tiles(focal_stats_multi_kernel, g, 3, (cudaStream_t)s, kFocalFused, tmap, mask, planes,
+                            out_pitch / 4, g);
     }
     // single statistic, or a raster TMA cannot describe: one launch per plane
     for (int i = 0; i < n_stats; ++i) {

@@ -5,33 +5,28 @@
 // them to float32 in registers (same rounding as astype: int -> f32 and f64 -> f32, round to nearest
 // even), then run the unchanged float32 operators.  For integer rasters the TMA unit can only
 // zero-fill out-of-raster cells, so the loader substitutes NaN from the cell coordinates.
-#include <math.h>
 #include <type_traits>
 
 #include "surface_ops.cuh"
 
 namespace xrs {
 
-bool make_tensor_map_2d_raw(CUtensorMap *map, const void *base, int64_t pitch_bytes, int64_t H, int64_t W,
-                            int dtype, int box_w, int box_h);  // lib_core.cu
-
 // The CTA-wide TMA pipeline of stencil3.cuh with a source element type TS != float: the ring holds the raw
 // cells (32-byte halos, as for float32: 16 cells of 2 bytes, 8 of int32, 4 of float64), consumer lanes convert.
 template <typename Op, typename TS, int ROWS, int STAGES, int WARPS, int CTAS>
-static int launch_ingest(const void *in, int dtype, int64_t in_pitch, const typename Op::Params &prm, float *out,
+static int launch_ingest(const void *in, int64_t in_pitch, const typename Op::Params &prm, float *out,
                          int64_t out_pitch, int64_t H, int64_t W, cudaStream_t stream) {
     static_assert(std::is_same<typename Op::in_t, float>::value, "ingest feeds float32 operators");
     CUtensorMap tmap;
-    const bool ok = (W % 4 == 0) && (out_pitch % 16 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) &&
-                    make_tensor_map_2d_raw(&tmap, in, in_pitch, H, W, dtype, kSubW, ROWS);
-    if (!ok) {
+    const bool out_aligned = out_pitch % 16 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    if (!strip_tma_map(&tmap, static_cast<const TS *>(in), in_pitch, H, W, ROWS, out_aligned)) {
         set_error("raster layout not supported by the direct-ingest path (needs 16-byte aligned rows, W %% 4 == 0)");
         return XRS_EUNSUPPORTED;
     }
     OutPtrs<Op> outs;
     outs.p[0] = out;
     outs.pitch_elems = out_pitch / 4;
-    return launch_tma<Op, ROWS, STAGES, WARPS, CTAS, TS>(tmap, prm, outs, H, W, stream, 2);  // 2 = direct-ingest TMA kernel
+    return launch_tma<Op, ROWS, STAGES, WARPS, CTAS, TS>(tmap, prm, outs, H, W, stream, kIngestTma);
 }
 
 // ring geometry: 2-byte cells need ROWS % 4 == 0 (128-byte aligned boxes); bytes in flight follow the
@@ -44,10 +39,10 @@ static int dispatch_dtype(const void *in, int dtype, int64_t in_pitch, const typ
                           int64_t out_pitch, int64_t H, int64_t W, cudaStream_t st) {
     constexpr int W_ = IngestCfg<Op>::kWarps, C_ = IngestCfg<Op>::kCtas;
     switch (dtype) {
-        case XRS_I16: return launch_ingest<Op, short, 4, 4, W_, C_>(in, dtype, in_pitch, prm, out, out_pitch, H, W, st);
-        case XRS_U16: return launch_ingest<Op, unsigned short, 4, 4, W_, C_>(in, dtype, in_pitch, prm, out, out_pitch, H, W, st);
-        case XRS_I32: return launch_ingest<Op, int, 4, 3, W_, C_>(in, dtype, in_pitch, prm, out, out_pitch, H, W, st);
-        case XRS_F64: return launch_ingest<Op, double, 2, 3, W_, C_>(in, dtype, in_pitch, prm, out, out_pitch, H, W, st);
+        case XRS_I16: return launch_ingest<Op, short, 4, 4, W_, C_>(in, in_pitch, prm, out, out_pitch, H, W, st);
+        case XRS_U16: return launch_ingest<Op, unsigned short, 4, 4, W_, C_>(in, in_pitch, prm, out, out_pitch, H, W, st);
+        case XRS_I32: return launch_ingest<Op, int, 4, 3, W_, C_>(in, in_pitch, prm, out, out_pitch, H, W, st);
+        case XRS_F64: return launch_ingest<Op, double, 2, 3, W_, C_>(in, in_pitch, prm, out, out_pitch, H, W, st);
     }
     set_error("direct ingest supports int16, uint16, int32 and float64 rasters");
     return XRS_EUNSUPPORTED;
@@ -66,11 +61,8 @@ extern "C" int xrs_surface_typed(int op, const void *in, int in_dtype, int64_t i
     switch (op) {
         case XRS_OP_SLOPE: {
             XRS_REQUIRE(p != nullptr, "cell sizes missing");
-            const double kx = 1.0 / (8.0 * p[0]), ky = 1.0 / (8.0 * p[1]);
-            SlopeOp::Params q;
-            q.rxy = kx / ky;
-            q.ky2 = (float)(ky * ky);
-            return dispatch_dtype<SlopeOp>(in, in_dtype, in_pitch, q, out, out_pitch, H, W, st);
+            return dispatch_dtype<SlopeOp>(in, in_dtype, in_pitch, SlopeParams::make(p[0], p[1]), out, out_pitch, H,
+                                           W, st);
         }
         case XRS_OP_ASPECT: {
             AspectOp::Params q = {0};
@@ -78,18 +70,13 @@ extern "C" int xrs_surface_typed(int op, const void *in, int in_dtype, int64_t i
         }
         case XRS_OP_CURVATURE: {
             XRS_REQUIRE(p != nullptr, "cell size missing");
-            CurvatureOp::Params q;
-            q.k = 100.0 / (p[0] * p[0]);
-            return dispatch_dtype<CurvatureOp>(in, in_dtype, in_pitch, q, out, out_pitch, H, W, st);
+            return dispatch_dtype<CurvatureOp>(in, in_dtype, in_pitch, CurvatureOp::Params::make(p[0]), out,
+                                               out_pitch, H, W, st);
         }
         case XRS_OP_HILLSHADE: {
             XRS_REQUIRE(p != nullptr, "azimuth / altitude missing");
-            const double az = 360.0 - p[0], azr = az * M_PI / 180., altr = p[1] * M_PI / 180., A = azr - M_PI / 2.;
-            HillshadeOp::Params q;
-            q.s0 = (float)sin(altr);
-            q.cy = (float)(0.5 * cos(altr) * cos(A));
-            q.cx = (float)(0.5 * cos(altr) * sin(A));
-            return dispatch_dtype<HillshadeOp>(in, in_dtype, in_pitch, q, out, out_pitch, H, W, st);
+            return dispatch_dtype<HillshadeOp>(in, in_dtype, in_pitch, HillshadeOp::Params::make(p[0], p[1]), out,
+                                               out_pitch, H, W, st);
         }
     }
     set_error("xrs_surface_typed serves slope, aspect, curvature and hillshade");

@@ -58,33 +58,14 @@ static encode_tiled_fn get_encode_fn() {
 }
 
 bool make_tensor_map_2d(CUtensorMap *map, const void *base, int64_t pitch_bytes, int64_t H, int64_t W,
-                        int elem_bytes, int box_w, int box_h) {
-    if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return false;
-    if (pitch_bytes % 16 != 0) return false;
-    if ((int64_t)box_w * elem_bytes % 16 != 0 || box_w > 256 || box_h > 256) return false;
-    encode_tiled_fn fn = get_encode_fn();
-    if (!fn) return false;
-    const cuuint64_t dims[2] = {(cuuint64_t)W, (cuuint64_t)H};
-    const cuuint64_t strides[1] = {(cuuint64_t)pitch_bytes};
-    const cuuint32_t box[2] = {(cuuint32_t)box_w, (cuuint32_t)box_h};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUtensorMapDataType dt = elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT64;
-    const CUresult r = fn(map, dt, 2, const_cast<void *>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NAN_REQUEST_ZERO_FMA);
-    return r == CUDA_SUCCESS;
-}
-
-// Raw-element tensor map for the direct-ingest kernels: dtype is an xrs_dtype; float64 gets the NaN
-// out-of-bounds fill, integer types are zero-filled by the hardware (the kernel patches NaN in).
-bool make_tensor_map_2d_raw(CUtensorMap *map, const void *base, int64_t pitch_bytes, int64_t H, int64_t W,
-                            int dtype, int box_w, int box_h) {
+                        xrs_dtype dtype, int box_w, int box_h) {
     CUtensorMapDataType dt;
     int esz;
     switch (dtype) {
-        case XRS_I16: case XRS_U16: dt = CU_TENSOR_MAP_DATA_TYPE_UINT16; esz = 2; break;
-        case XRS_I32: dt = CU_TENSOR_MAP_DATA_TYPE_INT32; esz = 4; break;
+        case XRS_F32: dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32; esz = 4; break;
         case XRS_F64: dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT64; esz = 8; break;
+        case XRS_I32: dt = CU_TENSOR_MAP_DATA_TYPE_INT32; esz = 4; break;
+        case XRS_I16: case XRS_U16: dt = CU_TENSOR_MAP_DATA_TYPE_UINT16; esz = 2; break;
         default: return false;
     }
     if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || pitch_bytes % 16 != 0) return false;
@@ -95,10 +76,21 @@ bool make_tensor_map_2d_raw(CUtensorMap *map, const void *base, int64_t pitch_by
     const cuuint64_t strides[1] = {(cuuint64_t)pitch_bytes};
     const cuuint32_t box[2] = {(cuuint32_t)box_w, (cuuint32_t)box_h};
     const cuuint32_t estr[2] = {1, 1};
-    const CUtensorMapFloatOOBfill fill =
-        dtype == XRS_F64 ? CU_TENSOR_MAP_FLOAT_OOB_FILL_NAN_REQUEST_ZERO_FMA : CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE;
+    const CUtensorMapFloatOOBfill fill = (dtype == XRS_F32 || dtype == XRS_F64)
+                                             ? CU_TENSOR_MAP_FLOAT_OOB_FILL_NAN_REQUEST_ZERO_FMA
+                                             : CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE;
     return fn(map, dt, 2, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, fill) == CUDA_SUCCESS;
+}
+
+int resident_ctas(const void *kernel, int threads, size_t smem, int max_per_sm, int64_t *resident) {
+    XRS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+    if (per_sm > max_per_sm) per_sm = max_per_sm;
+    if (per_sm < 1) per_sm = 1;
+    *resident = (int64_t)sm_count() * per_sm;
+    return XRS_OK;
 }
 
 }  // namespace xrs
@@ -130,7 +122,7 @@ int xrs_host_free(void *ptr) {
     return XRS_OK;
 }
 // test hook: which kernel the last launch on this thread chose (codes in xrs_b200.h)
-int xrs_debug_last_used_tma(void) { return xrs::last_launch_info().used_tma; }
+int xrs_debug_last_used_tma(void) { return xrs::last_launch_info().kind; }
 int xrs_debug_last_grid(void) { return xrs::last_launch_info().grid; }
 // test hook (host only, no device needed): the row-segment height the persistent kernels would pick
 int64_t xrs_debug_pick_seg_rows(int64_t H, int64_t n_tiles, int64_t resident, int64_t min_rows, int64_t lead,

@@ -13,7 +13,8 @@
 //     stream is steady and in raster order, and the bytes in flight per SM are set by the ring
 //     (ROWS x STAGES), not by how many warps the arithmetic needs.  An earlier pipeline, where every
 //     warp refilled its own 4-box ring after finishing a box, could not reach the copy rate even for
-//     an operator that does nothing (scripts/tune/tune3.cu compares the two);
+//     an operator that does nothing (the probe that compared the two, scripts/tune/tune3.cu, is in the
+//     git history);
 //   * out-of-raster cells are filled with NaN by the TMA unit, which is exactly the reference's
 //     raster-edge rule (NaN ring for the Horn family, NaN-skipping clamped windows for focal.mean);
 //   * the three input rows a cell needs are never re-read: operators keep per-row partial
@@ -29,8 +30,8 @@
 //     staging does not fit next to the ring (the 4-output suite) keep the register stores, chosen
 //     at compile time (TmaCfg::kBulk).
 // Rasters TMA cannot describe (width not a multiple of 4 cells, unaligned base / pitch) run a
-// per-warp ring filled by cp.async (stencil3_cpasync_kernel); a plain bounds-checked direct-load
-// kernel is kept as the reference implementation of the loader.  All three drive the very same
+// per-warp ring filled by cp.async (stencil3_cpasync_kernel), which fills its ring cell by cell with
+// bounds checks; the tests compare the TMA kernel with it bit for bit.  Both drive the very same
 // operator code.
 #pragma once
 #include "common.cuh"
@@ -85,21 +86,6 @@ template <typename T> __device__ __forceinline__ void load_cells4(const T *p, T 
     }
 }
 
-// Direct global loads with bounds checks (out-of-raster cells read as NaN): six independent scalar
-// loads per lane and row, so that several rows can be in flight at once.
-template <typename T>
-__device__ __forceinline__ Row6<T> load_row_direct(const T *in, int64_t pitch_elems, int64_t H,
-                                                   int64_t W, int64_t y, int64_t x) {
-    Row6<T> o;
-    const bool yin = (y >= 0) && (y < H);
-    const T *rp = in + (yin ? y : 0) * pitch_elems;
-    o.l = (yin && x >= 1 && x - 1 < W) ? __ldg(rp + x - 1) : nan_of<T>();
-#pragma unroll
-    for (int i = 0; i < 4; ++i) o.c[i] = (yin && (x + i) < W) ? __ldg(rp + x + i) : nan_of<T>();
-    o.r = (yin && (x + 4) < W) ? __ldg(rp + x + 4) : nan_of<T>();
-    return o;
-}
-
 template <typename TO> __device__ __forceinline__ void store4(TO *p, const Vec4<TO> &v, bool vec_ok,
                                                             int nvalid) {
     if (vec_ok && nvalid == 4) {
@@ -118,13 +104,7 @@ template <typename TO> __device__ __forceinline__ void store4(TO *p, const Vec4<
 
 template <typename TO> __device__ __forceinline__ void store4v(TO *p, const Vec4<TO> &v) {
     if constexpr (sizeof(TO) == 4) {
-#ifdef XRS_STORE_PLAIN
-        *reinterpret_cast<float4 *>(p) = make_float4(v.v[0], v.v[1], v.v[2], v.v[3]);
-#elif defined(XRS_STORE_CG)
-        __stcg(reinterpret_cast<float4 *>(p), make_float4(v.v[0], v.v[1], v.v[2], v.v[3]));
-#else
         __stcs(reinterpret_cast<float4 *>(p), make_float4(v.v[0], v.v[1], v.v[2], v.v[3]));
-#endif
     } else {
         __stcs(reinterpret_cast<double2 *>(p), make_double2(v.v[0], v.v[1]));
         __stcs(reinterpret_cast<double2 *>(p + 2), make_double2(v.v[2], v.v[3]));
@@ -206,7 +186,6 @@ template <typename TI, typename TS> __device__ __forceinline__ void load_cells4_
 // Shared-memory plan of one TMA-kernel instantiation: the input ring, then (bulk-store epilogue) kOutBufs
 // staging buffers of ROWS x kTileW cells per output, then the mbarriers.  The bulk epilogue is used when
 // CTAS such CTAs fit in an SM's 228 KB (1 KB of it reserved per CTA); otherwise lanes store from registers.
-constexpr size_t kSmemPerSm = 228 * 1024, kSmemPerCtaMax = 227 * 1024, kSmemReservedPerCta = 1024;
 constexpr int kOutBufs = 2;
 
 template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, typename TS = typename Op::in_t,
@@ -426,49 +405,6 @@ stencil3_tma_kernel(const __grid_constant__ CUtensorMap tmap,
     }
 }
 
-// ----------------------------------------------------------------------------- direct kernel
-template <typename Op>
-__global__ void __launch_bounds__(kWarpsPerCta * 32)
-stencil3_direct_kernel(const typename Op::in_t *__restrict__ in, int64_t in_pitch_elems,
-                       const __grid_constant__ typename Op::Params prm, const OutPtrs<Op> outs,
-                       const StripGeom g,
-                       int vec_ok) {
-    using T = typename Op::in_t;
-    using TO = typename Op::out_t;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t n_tasks = (int64_t)g.n_strips * g.n_segs;
-    const int64_t total_warps = (int64_t)gridDim.x * kWarpsPerCta;
-    for (int64_t task = (int64_t)blockIdx.x * kWarpsPerCta + warp; task < n_tasks; task += total_warps) {
-        const int seg = (int)(task / g.n_strips), strip = (int)(task % g.n_strips);
-        const int64_t x0 = (int64_t)strip * kStripW;
-        const int64_t y0 = (int64_t)seg * g.seg_rows;
-        const int64_t y1 = min(y0 + (int64_t)g.seg_rows, g.H);
-        Op op(prm);
-        const int64_t xl = x0 + kLaneCells * lane;
-        const int nvalid = (int)max((int64_t)0, min((int64_t)4, g.W - xl));
-        // batches of kBatch rows: all loads of a batch are issued before the first row is consumed
-        // (software pipelining; the operator state update itself stays branch-free)
-        constexpr int kBatch = 4;
-        for (int64_t yb = y0 - 1; yb <= y1; yb += kBatch) {
-            Row6<T> rows[kBatch];
-#pragma unroll
-            for (int u = 0; u < kBatch; ++u) rows[u] = load_row_direct<T>(in, in_pitch_elems, g.H, g.W, yb + u, xl);
-#pragma unroll
-            for (int u = 0; u < kBatch; ++u) {
-                Vec4<TO> o[Op::kOutputs];
-                op.step(rows[u], o);
-                const int64_t yout = yb + u - 1;
-                if (yout >= y0 && yout < y1 && nvalid > 0) {
-#pragma unroll
-                    for (int k = 0; k < Op::kOutputs; ++k)
-                        if (outs.p[k] != nullptr)
-                            store4<TO>(outs.p[k] + yout * outs.pitch_elems + xl, o[k], vec_ok != 0, nvalid);
-                }
-            }
-        }
-    }
-}
-
 // ----------------------------------------------------------------------------- cp.async kernel
 // Same warp-strip pipeline for rasters TMA cannot describe (width not a multiple of 4 cells, base
 // or pitch not 16-byte aligned): the per-warp ring is filled with 4-/8-byte cp.async copies
@@ -621,36 +557,33 @@ inline TileGeom make_tile_geom(int64_t H, int64_t W, int tile_w, int rows, int64
 }
 
 // ROWS x STAGES = the TMA ring of the CTA-wide pipeline, WARPS consumer warps per CTA, CTAS CTAs per
-// SM: tuned per operator (surface.cu, scripts/tune/tune5.cu).  `kind` is what LaunchInfo::used_tma reports.
+// SM: tuned per operator (surface.cu, scripts/tune/tune5.cu).  `kind` is what LaunchInfo::kind reports.
 // BULK defaults to the bulk-store epilogue wherever its staging fits; the tuning harness also times the
 // register-store epilogue, and other halo widths PAD.
 template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, typename TS = typename Op::in_t,
           int PAD = SrcPad<TS>::value, bool BULK = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, TS, PAD>::kBulk>
 int launch_tma(const CUtensorMap &tmap, const typename Op::Params &prm, const OutPtrs<Op> &outs, int64_t H,
-               int64_t W, cudaStream_t stream, int kind) {
+               int64_t W, cudaStream_t stream, LaunchKind kind) {
     using Cfg = TmaCfg<Op, ROWS, STAGES, WARPS, CTAS, TS, PAD>;
     static_assert(!BULK || Cfg::kBulk, "the bulk-store staging does not fit next to this ring");
     constexpr size_t smem = BULK ? Cfg::kBulkSmem : Cfg::kRegSmem;
     constexpr int threads = (WARPS + 1 + (BULK ? 1 : 0)) * 32;  // consumers, producer[, store warp]
     auto kern = stencil3_tma_kernel<Op, ROWS, STAGES, WARPS, TS, PAD, BULK>;
-    XRS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // persistent grid: CTAS per SM (or what fits), never more CTAs than tasks
-    int per_sm = 0;
-    XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
-    if (per_sm < 1) per_sm = 1;
-    if (per_sm > CTAS) per_sm = CTAS;
-    const int64_t resident = (int64_t)sm_count() * per_sm;
+    int64_t resident;
+    if (const int rc = resident_ctas(kern, threads, smem, CTAS, &resident)) return rc;
     const TileGeom g = make_tile_geom(H, W, Cfg::kTileW, ROWS, resident);
     const int64_t n_tasks = (int64_t)g.n_tiles * g.n_segs;
-    const int64_t grid = resident < n_tasks ? resident : n_tasks;
-    LaunchInfo &li = last_launch_info();
-    li.used_tma = kind;
-    li.grid = (int)grid;
-    li.block = threads;
-    li.smem_bytes = (int)smem;
-    kern<<<(unsigned)grid, threads, smem, stream>>>(tmap, prm, outs, g);
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    return launch(kern, resident < n_tasks ? resident : n_tasks, threads, smem, stream, kind, tmap, prm, outs, g);
+}
+
+// The TMA strip kernel takes a raster when W % 4 == 0 (a lane's 4 cells are all inside or all outside), the
+// output rows are 16-byte aligned (bulk copies and float4 stores) and TMA can describe the input; then `map`
+// holds the input's tensor map.
+template <typename TS>
+bool strip_tma_map(CUtensorMap *map, const TS *in, int64_t in_pitch_bytes, int64_t H, int64_t W, int rows,
+                   bool out_aligned) {
+    return out_aligned && W % 4 == 0 && make_tensor_map_2d(map, in, in_pitch_bytes, H, W, dtype_of<TS>(), kSubW, rows);
 }
 
 constexpr int kFallbackRows = 4, kFallbackStages = 4;  // cp.async ring (per warp)
@@ -682,20 +615,16 @@ int launch_stencil3(const typename Op::in_t *in, int64_t in_pitch_bytes, const t
     XRS_REQUIRE(any, "no output pointer given");
     outs.pitch_elems = out_pitch_bytes / (int64_t)sizeof(TO);
 
-    const int sms = sm_count();
-    LaunchInfo &li = last_launch_info();
-
     CUtensorMap tmap;
-    const bool tma_ok = out_vec_ok && (W % 4 == 0) &&
-                        make_tensor_map_2d(&tmap, in, in_pitch_bytes, H, W, (int)sizeof(T), kSubW, ROWS);
-    if (tma_ok) return launch_tma<Op, ROWS, STAGES, WARPS, CTAS>(tmap, prm, outs, H, W, stream, 1);
+    if (strip_tma_map(&tmap, in, in_pitch_bytes, H, W, ROWS, out_vec_ok))
+        return launch_tma<Op, ROWS, STAGES, WARPS, CTAS>(tmap, prm, outs, H, W, stream, kStripTma);
     {  // rasters TMA cannot describe: the per-warp cp.async ring
         constexpr int FR = sizeof(T) == 8 ? 2 : kFallbackRows, FS = kFallbackStages;
         StripGeom g;
         g.H = H;
         g.W = W;
         g.n_strips = (int)((W + kStripW - 1) / kStripW);
-        const int64_t resident_warps = (int64_t)sms * 2 * kWarpsPerCta;
+        const int64_t resident_warps = (int64_t)sm_count() * 2 * kWarpsPerCta;
         int64_t want_segs = (resident_warps * 8 + g.n_strips - 1) / g.n_strips;
         int64_t seg_rows = (H + want_segs - 1) / (want_segs > 0 ? want_segs : 1);
         if (seg_rows < 64) seg_rows = 64;
@@ -708,22 +637,11 @@ int launch_stencil3(const typename Op::in_t *in, int64_t in_pitch_bytes, const t
         const int64_t ctas_needed = (n_tasks + kWarpsPerCta - 1) / kWarpsPerCta;
         constexpr size_t smem = (size_t)kWarpsPerCta * FS * FR * kBoxW * sizeof(T);
         auto kern = stencil3_cpasync_kernel<Op, FR, FS>;
-        XRS_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 0;
-        XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kWarpsPerCta * 32, smem));
-        if (per_sm < 1) per_sm = 1;
-        if (per_sm > 2) per_sm = 2;
-        int64_t grid = (int64_t)sms * per_sm;
-        if (grid > ctas_needed) grid = ctas_needed;
-        li.used_tma = 0;
-        li.grid = (int)grid;
-        li.block = kWarpsPerCta * 32;
-        li.smem_bytes = (int)smem;
-        kern<<<(unsigned)grid, kWarpsPerCta * 32, smem, stream>>>(in, in_pitch_bytes / (int64_t)sizeof(T), prm, outs, g,
-                                                                out_vec_ok ? 1 : 0);
+        int64_t resident;
+        if (const int rc = resident_ctas(kern, kWarpsPerCta * 32, smem, 2, &resident)) return rc;
+        return launch(kern, resident < ctas_needed ? resident : ctas_needed, kWarpsPerCta * 32, smem, stream,
+                      kStripCpAsync, in, in_pitch_bytes / (int64_t)sizeof(T), prm, outs, g, out_vec_ok ? 1 : 0);
     }
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
 }
 
 }  // namespace xrs

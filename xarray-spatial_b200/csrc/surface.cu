@@ -1,7 +1,5 @@
 // surface.cu -- C-ABI entry points of the 3x3 family (slope, aspect, curvature, hillshade,
 // fused suite, focal.mean).  Argument checking and launch geometry live in stencil3.cuh.
-#include <math.h>
-
 #include "surface_ops.cuh"
 
 using namespace xrs;
@@ -23,27 +21,6 @@ using namespace xrs;
 #define XRS_CFG_SUITE 8, 2, 12, 1     /* ~145 registers per thread: one 12-warp CTA per SM, register stores */
 #define XRS_CFG_F64 2, 4, 16, 1       /* 8-byte cells: focal.mean f64 */
 #define XRS_CFG_F32_F64 2, 4, 16, 1   /* float32 in, float64 out (12 B/cell) */
-
-static SlopeOp::Params slope_params(double cellsize_x, double cellsize_y) {
-    const double kx = 1.0 / (8.0 * cellsize_x), ky = 1.0 / (8.0 * cellsize_y);
-    SlopeOp::Params p;
-    p.rxy = kx / ky;
-    p.ky2 = (float)(ky * ky);
-    return p;
-}
-
-static HillshadeOp::Params hillshade_params(double azimuth, double angle_altitude) {
-    // hillshade.py:23-27: azimuth = 360 - azimuth; rad conversions in Python float (f64)
-    const double az = 360.0 - azimuth;
-    const double azimuthrad = az * M_PI / 180.;
-    const double altituderad = angle_altitude * M_PI / 180.;
-    const double A = azimuthrad - M_PI / 2.;
-    HillshadeOp::Params p;
-    p.s0 = (float)sin(altituderad);
-    p.cy = (float)(0.5 * cos(altituderad) * cos(A));
-    p.cx = (float)(0.5 * cos(altituderad) * sin(A));
-    return p;
-}
 
 // 3x3 kernels of convolve_2d take the warp-strip path (called from conv.cu)
 int xrs_conv3_strip(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
@@ -81,7 +58,7 @@ extern "C" {
 
 int xrs_slope_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
                   double cellsize_x, double cellsize_y, xrs_stream_t s) {
-    const SlopeOp::Params p = slope_params(cellsize_x, cellsize_y);
+    const SlopeOp::Params p = SlopeParams::make(cellsize_x, cellsize_y);
     float *outs[1] = {out};
     if (p.rxy == 1.0)  // square cells: same arithmetic minus the multiplication by 1
         return launch_stencil3<SlopeSqOp, XRS_CFG_SLOPE_SQ>(in, in_pitch, p, outs, out_pitch, H, W, (cudaStream_t)s);
@@ -99,8 +76,7 @@ int xrs_aspect_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pi
 
 int xrs_curvature_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H,
                       int64_t W, double cellsize, xrs_stream_t s) {
-    CurvatureOp::Params p;
-    p.k = 100.0 / (cellsize * cellsize);
+    const CurvatureOp::Params p = CurvatureOp::Params::make(cellsize);
     float *outs[1] = {out};
     return launch_stencil3<CurvatureOp, XRS_CFG_LIGHT>(in, in_pitch, p, outs, out_pitch, H, W,
                                                               (cudaStream_t)s);
@@ -108,7 +84,7 @@ int xrs_curvature_f32(const float *in, int64_t in_pitch, float *out, int64_t out
 
 int xrs_hillshade_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H,
                       int64_t W, double azimuth, double angle_altitude, xrs_stream_t s) {
-    const HillshadeOp::Params p = hillshade_params(azimuth, angle_altitude);
+    const HillshadeOp::Params p = HillshadeOp::Params::make(azimuth, angle_altitude);
     float *outs[1] = {out};
     return launch_stencil3<HillshadeOp, XRS_CFG_LIGHT>(in, in_pitch, p, outs, out_pitch, H, W,
                                                               (cudaStream_t)s);
@@ -119,10 +95,9 @@ int xrs_surface_suite_f32(const float *in, int64_t in_pitch, float *slope_out, f
                           int64_t W, double cellsize_x, double cellsize_y, double azimuth,
                           double angle_altitude, xrs_stream_t s) {
     SuiteOp::Params p;
-    p.slope = slope_params(cellsize_x, cellsize_y);
-    const double cs = (cellsize_x + cellsize_y) / 2;  // curvature.py:234
-    p.curv.k = 100.0 / (cs * cs);
-    p.hill = hillshade_params(azimuth, angle_altitude);
+    p.slope = SlopeParams::make(cellsize_x, cellsize_y);
+    p.curv = CurvatureOp::Params::make((cellsize_x + cellsize_y) / 2);  // curvature.py:234
+    p.hill = HillshadeOp::Params::make(azimuth, angle_altitude);
     float *outs[4] = {slope_out, aspect_out, curvature_out, hillshade_out};
     if (p.slope.rxy == 1.0)
         return launch_stencil3<SuiteSqOp, XRS_CFG_SUITE>(in, in_pitch, p, outs, out_pitch, H, W, (cudaStream_t)s);

@@ -7,6 +7,8 @@
 // tail (sqrt / atan / atan2) is evaluated in f32 on the correctly-rounded f64 intermediate,
 // which keeps the result within ~3e-7 relative of the oracle (bar: 1e-5).
 #pragma once
+#include <math.h>
+
 #include "stencil3.cuh"
 
 namespace xrs {
@@ -37,6 +39,13 @@ __device__ __forceinline__ HornRow horn_row(const Row6<float> &r) {
 struct SlopeParams {
     double rxy;  // (1/(8 csx)) / (1/(8 csy)) = csy / csx
     float ky2;   // (1/(8 csy))^2
+    static SlopeParams make(double cellsize_x, double cellsize_y) {
+        const double kx = 1.0 / (8.0 * cellsize_x), ky = 1.0 / (8.0 * cellsize_y);
+        SlopeParams p;
+        p.rxy = kx / ky;
+        p.ky2 = (float)(ky * ky);
+        return p;
+    }
 };
 // p = dz_dx^2 + dz_dy^2 = ky^2 ((X kx/ky)^2 + Y^2): X, Y are exact in f64, the sum of squares
 // is formed in f64 and only then rounded to f32 (the result needs f32 accuracy).
@@ -124,6 +133,11 @@ struct CurvatureOp {
     static constexpr int kOutputs = 1;
     struct Params {
         double k;  // 100 / cellsize^2
+        static Params make(double cellsize) {
+            Params p;
+            p.k = 100.0 / (cellsize * cellsize);
+            return p;
+        }
     };
     const Params &p;
     float n2[4];      // row y-2 centre cells
@@ -164,6 +178,18 @@ struct HillshadeOp {
     static constexpr int kOutputs = 1;
     struct Params {
         float s0, cy, cx;  // sin(alt), 0.5*cos(alt)*cos(A), 0.5*cos(alt)*sin(A)
+        static Params make(double azimuth, double angle_altitude) {
+            // hillshade.py:23-27: azimuth = 360 - azimuth; rad conversions in Python float (f64)
+            const double az = 360.0 - azimuth;
+            const double azimuthrad = az * M_PI / 180.;
+            const double altituderad = angle_altitude * M_PI / 180.;
+            const double A = azimuthrad - M_PI / 2.;
+            Params p;
+            p.s0 = (float)sin(altituderad);
+            p.cy = (float)(0.5 * cos(altituderad) * cos(A));
+            p.cx = (float)(0.5 * cos(altituderad) * sin(A));
+            return p;
+        }
     };
     const Params &p;
     float n2[4];

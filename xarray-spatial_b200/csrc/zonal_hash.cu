@@ -689,17 +689,12 @@ template <typename VT, typename ZT, bool ZP = false> static int launch_zh(const 
     const int64_t H = a.n / a.W;
     const int64_t n_tasks = ((a.W + 127) / 128) * ((H + kZhSegRows - 1) / kZhSegRows);
     constexpr size_t smem = ZhTable<VT>::kBytes;
-    XRS_CUDA(cudaFuncSetAttribute(zonal_hash_kernel<VT, ZT, ZP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    XRS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, zonal_hash_kernel<VT, ZT, ZP>, kZhThreads, smem));
-    if (per_sm < 1) per_sm = 1;
-    int64_t grid = (int64_t)sm_count() * per_sm;
+    int64_t grid;   // as many CTAs as fit, no cap per SM
+    if (const int rc = resident_ctas(zonal_hash_kernel<VT, ZT, ZP>, kZhThreads, smem, INT_MAX, &grid)) return rc;
     const int64_t need = (n_tasks + kZhThreads / 32 - 1) / (kZhThreads / 32);
     if (grid > need) grid = need;
     if (grid < 1) grid = 1;
-    zonal_hash_kernel<VT, ZT, ZP><<<(unsigned)grid, kZhThreads, smem, s>>>(a);
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    return launch(zonal_hash_kernel<VT, ZT, ZP>, grid, kZhThreads, smem, s, kZonalHash, a);
 }
 
 }  // namespace xrs
