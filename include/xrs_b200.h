@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define XRS_ABI_VERSION 1
+#define XRS_ABI_VERSION 2
 
 typedef void *xrs_stream_t; /* cudaStream_t */
 
@@ -179,28 +179,17 @@ int xrs_ebbi_f32(const float *red, const float *swir, const float *tir, float *o
  * zones (zones_dtype: I32, I64, F32, F64) and values (values_dtype: F32, F64) are device arrays of n
  * cells; a cell contributes to its zone if its value is finite and != nodata (when has_nodata). */
 
-/* The group-by: aggregation into an open-addressing
- * hash table of `cap` slots (power of two >= 1024; device arrays keys/count/s1/s2/vmin/vmax of
- * `cap` entries, initialised by xrs_zonal_hash_init).  keys[slot] is the zone id (int64 for
- * integer zones, the bit pattern of the float64 value for float zones; INT64_MIN = empty, so an int64
- * zone INT64_MIN is not counted here -- xrs_zonal_hash_run reports it),
- * s1/s2 are sums of (v - pivot) and (v - pivot)^2.  Every finite zone value present in the
- * raster gets a slot, also when none of its cells is valid (count 0).  *overflow (device
- * int) is set when the raster holds more than `cap` distinct zones.  row_len is the raster's
- * row length (n = rows * row_len): the scan walks down 128-column strips so that runs of equal
- * zone ids stay long. */
-int xrs_zonal_hash_init(int64_t *keys, int64_t *count, double *s1, double *s2, double *vmin,
-                        double *vmax, int cap, int *overflow, xrs_stream_t s);
-int xrs_zonal_hash_accumulate(const void *values, int values_dtype, const void *zones,
-                              int zones_dtype, int64_t n, int64_t row_len, double pivot, int has_nodata,
-                              double nodata, int64_t *keys, int64_t *count, double *s1,
-                              double *s2, double *vmin, double *vmax, int cap, int *overflow,
-                              xrs_stream_t s);
+/* The group-by: aggregation into an open-addressing hash table of `cap` slots (power of two >= 1024; device
+ * arrays keys/count/s1/s2/vmin/vmax of `cap` entries).  keys[slot] is the zone id (int64 for integer zones, the
+ * bit pattern of the float64 value for float zones; INT64_MIN = empty, so an int64 zone INT64_MIN is not
+ * counted in the table -- packed[3] reports it), s1/s2 are sums of (v - pivot) and (v - pivot)^2.  Every finite
+ * zone value present in the raster gets a slot, also when none of its cells is valid (count 0).  row_len is the
+ * raster's row length (n = rows * row_len): the scan walks down 128-column strips so that runs of equal zone ids
+ * stay long. */
 
-/* The whole single-pass group-by behind one call, with no host round trip in the middle: samples the
- * pivot on the device (median of 4096 strided samples, unless use_pivot_hint: row stripes must share one
- * pivot), initialises the table, accumulates, then compacts the used slots into `packed` (device,
- * 4 + 6 * max_out doubles):
+/* The first pass, with no host round trip in the middle: samples the pivot on the device (median of 4096
+ * strided samples, unless use_pivot_hint: row stripes must share one pivot), empties the table, accumulates,
+ * then compacts the used slots into `packed` (device, 4 + 6 * max_out doubles):
  *   packed[0] = used slots, packed[1] = table overflowed (grow `cap` and retry), packed[2] = pivot,
  *   packed[3] = an int64 zone INT64_MIN (the empty key, not in the table) was met: compute it apart,
  *   then 6 rows of max_out: key bit patterns, count (int64 bit patterns), s1, s2, min, max, in any
@@ -223,7 +212,8 @@ int xrs_zonal_hash_second_pass(const void *values, int values_dtype, const void 
                                double *vmax, int cap, double *packed, int max_out, int *flags, xrs_stream_t s);
 
 /* `majority` (zonal.py:56-68): counts (zone, value) pairs of float32 values / int32 zones into
- * a hash table (keys/count of `cap` entries, initialised with xrs_zonal_hash_init; key =
+ * a hash table (keys/count of `cap` entries, emptied here; *overflow (device int) is set when it holds
+ * fewer slots than the raster has distinct pairs; key =
  * (zone << 32) | (float32 bits of the value ^ 0x7fc00000), -0.0 folded into +0.0; the XOR makes the
  * empty key INT64_MIN stand for (zone INT32_MIN, a NaN), a pair never counted).  The caller picks the most
  * frequent value per zone (smallest value on ties). */
@@ -272,7 +262,7 @@ int xrs_host_free(void *ptr);
  * kernel, 1 TMA strip kernel, 2 direct-ingest TMA kernel, 3 running-box kernel (uniform convolve_2d, focal.apply
  * mean over an all-ones window), 4 generic tiled convolve, 5 bounds-checked convolve fallback, 6 fused focal
  * statistics, 7 tiled single focal statistic, 8 bounds-checked focal statistic fallback, 9 zonal group-by
- * (xrs_zonal_hash_accumulate / _run / _second_pass) -- and with how many CTAs */
+ * (xrs_zonal_hash_run / _second_pass), 10 zonal pair count (xrs_zonal_pair_count) -- and with how many CTAs */
 int xrs_debug_last_used_tma(void);
 int xrs_debug_last_grid(void);
 /* host-only test hook: the row-segment height the persistent kernels pick for a raster of H rows cut into

@@ -109,7 +109,7 @@ from xrspatial_b200 import zonal as Z  # noqa: E402
 zt, vt = zones, dem
 sel = np.arange(1024, dtype=np.int32)
 add("zonal hash partials (ids discovered)", timeit(lambda: Z.hash_partials(zt, vt)), 8,
-    note="xrs_zonal_hash_accumulate + compaction + tiny D2H")
+    note="xrs_zonal_hash_run: pivot, accumulation, compaction + tiny D2H")
 hz = ((torch.arange(side, device="cuda", dtype=torch.int64)[:, None] * 7919 +
        torch.arange(side, device="cuda", dtype=torch.int64)[None, :] * 104729) % 1024).to(torch.int32)
 add("zonal hash partials, scattered zones", timeit(lambda: Z.hash_partials(hz, vt), n=3), 8,

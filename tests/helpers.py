@@ -6,7 +6,7 @@ import numpy as np
 
 # what xrs_debug_last_used_tma reports (LaunchKind in csrc/common.cuh)
 (K_STRIP_CPASYNC, K_STRIP_TMA, K_INGEST, K_BOX, K_CONV_TILED, K_CONV_DIRECT, K_FUSED, K_STAT_TILED, K_STAT_DIRECT,
- K_ZONAL) = range(10)
+ K_ZONAL, K_ZONAL_PAIR) = range(11)
 
 SENTINEL = 0x5A
 

@@ -25,12 +25,12 @@ def test_header_declares_the_hot_path():
         assert s in syms
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_at_abi_version_2():
     import xrspatial_b200
     lib = xrspatial_b200._lib.lib()
     for s in header_symbols():
         assert hasattr(lib, s), "libxrs_b200.so does not export %s" % s
-    assert lib.xrs_abi_version() == 1
+    assert lib.xrs_abi_version() == 2
 
 
 def test_ctypes_prototypes_cover_the_header():

@@ -843,7 +843,7 @@ def test_zonal_custom_stats(xb, known, refout):
                                        rtol=2e-6, err_msg=c)
 
 
-def test_majority_by_sort_equals_the_pair_table(xb):
+def test_majority_by_sort_equals_the_pair_table(xb, monkeypatch):
     """`majority` has two engines: the (zone, value) pair-count kernel (int32 zones, float32-exact
     values) and one device sort (everything else: wide / non-integer zone ids, float64 values,
     continuous rasters that overflow the pair table).  Same answers, incl. NaN, nodata and -0.0."""
@@ -873,12 +873,13 @@ def test_majority_by_sort_equals_the_pair_table(xb):
     # continuous values through the public API: the pair table overflows its (small here) budget
     vals = rng.standard_normal((64, 4096)).astype(np.float32)
     zz = (np.arange(64)[:, None] // 16 * 2 + np.arange(4096)[None, :] // 2048).astype(np.int32)
-    old = Z.pair_counts.__defaults__
-    Z.pair_counts.__defaults__ = (None, None, 1 << 10, 1 << 12)
-    try:
-        df = xb.zonal_stats(da(xb, dev(zz)), da(xb, dev(vals)), stats_funcs=["majority"])
-    finally:
-        Z.pair_counts.__defaults__ = old
+    monkeypatch.setattr(Z, "_PAIR_CAP", 1 << 10)
+    monkeypatch.setattr(Z, "_MAJORITY_PAIR_MAX_CAP", 1 << 12)
+    sorts = []
+    by_sort = Z._majority_by_sort
+    monkeypatch.setattr(Z, "_majority_by_sort", lambda *a: sorts.append(a[2]) or by_sort(*a))
+    df = xb.zonal_stats(da(xb, dev(zz)), da(xb, dev(vals)), stats_funcs=["majority"])
+    assert sorts == [8], "the pair table did not overflow into the sort"
     ref = o.zonal_stats(zz, vals, stats_funcs=["majority"])
     np.testing.assert_array_equal(np.asarray(df["majority"]), np.asarray(ref["majority"], dtype=np.float64))
 

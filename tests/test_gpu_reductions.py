@@ -18,7 +18,7 @@ import numpy as np
 import pytest
 
 import oracle as o
-from helpers import terrain
+from helpers import K_ZONAL_PAIR, terrain
 
 pytestmark = pytest.mark.gpu
 
@@ -285,6 +285,7 @@ def test_majority_and_crosstab_with_the_int32_min_zone(xb, zdt):
             row = np.asarray(df["zone"]) == np.iinfo(np.int32).min
             assert np.asarray(df["majority"])[row][0] == 0.0
         ct = xb.zonal_crosstab(da(xb, dev(zones)), da(xb, dev(v)))
+        assert xb._lib.lib().xrs_debug_last_used_tma() == K_ZONAL_PAIR
         rc = o.crosstab(zones, v)
         np.testing.assert_array_equal(np.asarray(ct["zone"]), rc["zone"])
         cats = [c for c in rc if c != "zone"]

@@ -55,8 +55,6 @@ def _declare(lib):
         "xrs_gci_f32": [P, P, P, I64, P],
         "xrs_sipi_f32": [P, P, P, P, I64, P],
         "xrs_ebbi_f32": [P, P, P, P, I64, P],
-        "xrs_zonal_hash_init": [P, P, P, P, P, P, I, P, P],
-        "xrs_zonal_hash_accumulate": [P, I, P, I, I64, I64, D, I, D, P, P, P, P, P, P, I, P, P],
         "xrs_zonal_hash_run": [P, I, P, I, I64, I64, I, D, I, D, P, P, P, P, P, P, I, P, I, P, P],
         "xrs_zonal_hash_second_pass": [P, I, P, I, I64, I64, I, D, P, P, P, P, P, P, P, I, P, I, P, P],
         "xrs_zonal_pair_count": [P, P, I64, I64, I, D, P, P, I, P, P],

@@ -29,6 +29,7 @@ enum LaunchKind : int {
     kFocalTiled = 7,    // tiled single focal statistic
     kFocalDirect = 8,   // bounds-checked single focal statistic
     kZonalHash = 9,     // zonal group-by
+    kZonalPair = 10,    // zonal (zone, value) pair count
 };
 
 struct LaunchInfo {  // for tests / profiling: what the last launch on this thread chose

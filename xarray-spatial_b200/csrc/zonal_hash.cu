@@ -13,6 +13,8 @@
 // 8 algorithmic bytes per cell (f32 values + i32 zones): HBM-bound.
 #include <math.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace xrs {
@@ -595,25 +597,15 @@ __global__ void __launch_bounds__(kZhThreads) zonal_pair_kernel(const __grid_con
     }
 }
 
-__global__ void zonal_hash_init_kernel(long long *keys, unsigned long long *count, double *s1, double *s2,
-                                       double *vmin, double *vmax, int cap, int *overflow) {
+// Empties `cap` slots: keys to the empty key unless `keys` is NULL (the second pass keeps the first pass's keys),
+// counts to 0, and the sums and min / max to their identities unless `s1` is NULL (the pair table has none).
+__global__ void zonal_table_init_kernel(long long *keys, unsigned long long *count, double *s1, double *s2,
+                                        double *vmin, double *vmax, int cap) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < cap) {
-        keys[i] = kZhEmpty;
-        count[i] = 0ull;
-        s1[i] = 0.0; s2[i] = 0.0; vmin[i] = INFINITY; vmax[i] = -INFINITY;
-    }
-    if (i == 0) *overflow = 0;
-}
-
-// accumulators back to empty, keys kept (second pass over a populated table)
-__global__ void zonal_hash_reset_kernel(unsigned long long *count, double *s1, double *s2, double *vmin, double *vmax,
-                                        int cap) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < cap) {
-        count[i] = 0ull;
-        s1[i] = 0.0; s2[i] = 0.0; vmin[i] = INFINITY; vmax[i] = -INFINITY;
-    }
+    if (i >= cap) return;
+    if (keys) keys[i] = kZhEmpty;
+    count[i] = 0ull;
+    if (s1) { s1[i] = 0.0; s2[i] = 0.0; vmin[i] = INFINITY; vmax[i] = -INFINITY; }
 }
 
 // ---- one-call front end: pivot sampling, table compaction and header, all on the device ----------
@@ -685,16 +677,73 @@ __global__ void zonal_flags_kernel(int *flags, double *pivot_dev, double pivot_h
     if (pivot_dev) *pivot_dev = pivot_hint;
 }
 
-template <typename VT, typename ZT, bool ZP = false> static int launch_zh(const ZhArgs &a, cudaStream_t s) {
-    const int64_t H = a.n / a.W;
-    const int64_t n_tasks = ((a.W + 127) / 128) * ((H + kZhSegRows - 1) / kZhSegRows);
+// CTAs that give every warp of a zonal kernel a task: 128-column x kZhSegRows-row tasks, 8 warps per CTA
+static int64_t zh_ctas_for_tasks(int64_t n, int64_t W) {
+    const int64_t n_tasks = ((W + 127) / 128) * ((n / W + kZhSegRows - 1) / kZhSegRows);
+    return (n_tasks + kZhThreads / 32 - 1) / (kZhThreads / 32);
+}
+
+// zonal_hash_kernel for one pass: as many CTAs as fit (no cap per SM), no more than there are tasks
+template <typename VT, typename ZT> static int launch_zh(const ZhArgs &a, bool second, cudaStream_t s) {
+    const auto kernel = second ? &zonal_hash_kernel<VT, ZT, true> : &zonal_hash_kernel<VT, ZT, false>;
     constexpr size_t smem = ZhTable<VT>::kBytes;
-    int64_t grid;   // as many CTAs as fit, no cap per SM
-    if (const int rc = resident_ctas(zonal_hash_kernel<VT, ZT, ZP>, kZhThreads, smem, INT_MAX, &grid)) return rc;
-    const int64_t need = (n_tasks + kZhThreads / 32 - 1) / (kZhThreads / 32);
-    if (grid > need) grid = need;
-    if (grid < 1) grid = 1;
-    return launch(zonal_hash_kernel<VT, ZT, ZP>, grid, kZhThreads, smem, s, kZonalHash, a);
+    int64_t grid;
+    if (const int rc = resident_ctas(kernel, kZhThreads, smem, INT_MAX, &grid)) return rc;
+    grid = std::max<int64_t>(1, std::min(grid, zh_ctas_for_tasks(a.n, a.W)));
+    return launch(kernel, grid, kZhThreads, smem, s, kZonalHash, a);
+}
+template <typename VT> static int launch_zh(const ZhArgs &a, int zones_dtype, bool second, cudaStream_t s) {
+    switch (zones_dtype) {
+        case XRS_I32: return launch_zh<VT, int>(a, second, s);
+        case XRS_I64: return launch_zh<VT, long long>(a, second, s);
+        case XRS_F32: return launch_zh<VT, float>(a, second, s);
+        default: return launch_zh<VT, double>(a, second, s);
+    }
+}
+
+// The used slots and the pass's flags into `packed` (layout in xrs_b200.h).
+static int zh_compact(const ZhArgs &a, double *packed, int max_out, int *flags, cudaStream_t s) {
+    zonal_compact_kernel<<<(a.cap + 255) / 256, 256, 0, s>>>(a.keys, a.count, a.s1, a.s2, a.vmin, a.vmax, a.cap, packed,
+                                                             max_out, flags);
+    zonal_header_kernel<<<1, 1, 0, s>>>(packed, flags, packed + 2);
+    XRS_CUDA(cudaGetLastError());
+    return XRS_OK;
+}
+
+// One group-by pass with everything it enqueues.  First pass: samples the pivot (unless use_pivot_hint) and
+// empties the table.  Second pass: resets the accumulators, keeps the first pass's keys and sums about
+// zone_pivots[slot].  Then both accumulate and compact.
+static int zh_pass(bool second, const void *values, int values_dtype, const void *zones, int zones_dtype, int64_t n,
+                   int64_t row_len, int has_nodata, double nodata, int use_pivot_hint, double pivot_hint,
+                   const double *zone_pivots, int64_t *keys, int64_t *count, double *s1, double *s2, double *vmin,
+                   double *vmax, int cap, double *packed, int max_out, int *flags, cudaStream_t st) {
+    XRS_REQUIRE(values && zones && keys && count && s1 && s2 && vmin && vmax && packed && flags &&
+                    (zone_pivots || !second),
+                "NULL pointer");
+    XRS_REQUIRE(values_dtype == XRS_F32 || values_dtype == XRS_F64, "values must be float32 or float64");
+    XRS_REQUIRE(zones_dtype >= XRS_F32 && zones_dtype <= XRS_I64, "unknown zones dtype");
+    XRS_REQUIRE(cap >= 1024 && (cap & (cap - 1)) == 0, "cap must be a power of two >= 1024");
+    XRS_REQUIRE(max_out >= 1, "max_out must be positive");
+    XRS_REQUIRE(n >= 1 && row_len >= 1 && n % row_len == 0, "n must be a positive multiple of row_len");
+    double *pivot_dev = packed + 2;   // the header's pivot cell doubles as the device-side pivot
+    zonal_flags_kernel<<<1, 1, 0, st>>>(flags, pivot_dev, pivot_hint);
+    if (!use_pivot_hint) {
+        if (values_dtype == XRS_F32) zonal_pivot_kernel<float><<<1, 256, 0, st>>>((const float *)values, n, pivot_dev);
+        else zonal_pivot_kernel<double><<<1, 256, 0, st>>>((const double *)values, n, pivot_dev);
+    }
+    zonal_table_init_kernel<<<(cap + 255) / 256, 256, 0, st>>>(second ? nullptr : (long long *)keys,
+                                                               (unsigned long long *)count, s1, s2, vmin, vmax, cap);
+    XRS_CUDA(cudaGetLastError());
+    ZhArgs a;
+    a.values = values; a.zones = zones; a.n = n; a.W = row_len;
+    a.pivot = 0.0; a.pivot_ptr = second ? nullptr : pivot_dev; a.zone_pivots = zone_pivots;
+    a.has_nodata = has_nodata; a.nodata = nodata;
+    a.keys = (long long *)keys; a.count = (unsigned long long *)count; a.s1 = s1; a.s2 = s2; a.vmin = vmin;
+    a.vmax = vmax; a.cap = cap; a.overflow = flags; a.sentinel = flags + 2;
+    const int rc = values_dtype == XRS_F32 ? launch_zh<float>(a, zones_dtype, second, st)
+                                           : launch_zh<double>(a, zones_dtype, second, st);
+    if (rc != XRS_OK) return rc;
+    return zh_compact(a, packed, max_out, flags, st);
 }
 
 }  // namespace xrs
@@ -703,149 +752,42 @@ using namespace xrs;
 
 extern "C" {
 
-int xrs_zonal_hash_init(int64_t *keys, int64_t *count, double *s1, double *s2, double *vmin, double *vmax, int cap,
-                        int *overflow, xrs_stream_t s) {
-    XRS_REQUIRE(keys && count && s1 && s2 && vmin && vmax && overflow, "NULL pointer");
-    XRS_REQUIRE(cap >= 1024 && (cap & (cap - 1)) == 0, "cap must be a power of two >= 1024");
-    zonal_hash_init_kernel<<<(cap + 255) / 256, 256, 0, (cudaStream_t)s>>>(
-        (long long *)keys, (unsigned long long *)count, s1, s2, vmin, vmax, cap, overflow);
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
-}
-
-int xrs_zonal_hash_accumulate(const void *values, int values_dtype, const void *zones, int zones_dtype, int64_t n,
-                              int64_t row_len, double pivot, int has_nodata, double nodata, int64_t *keys, int64_t *count,
-                              double *s1, double *s2, double *vmin, double *vmax, int cap, int *overflow,
-                              xrs_stream_t s) {
-    if (n <= 0) return XRS_OK;
-    XRS_REQUIRE(values && zones && keys && count && s1 && s2 && vmin && vmax && overflow, "NULL pointer");
-    XRS_REQUIRE(values_dtype == XRS_F32 || values_dtype == XRS_F64, "values must be float32 or float64");
-    XRS_REQUIRE(zones_dtype >= XRS_F32 && zones_dtype <= XRS_I64, "unknown zones dtype");
-    XRS_REQUIRE(cap >= 1024 && (cap & (cap - 1)) == 0, "cap must be a power of two >= 1024");
-    XRS_REQUIRE(row_len >= 1 && n % row_len == 0, "n must be a multiple of row_len");
-    ZhArgs a;
-    a.values = values; a.zones = zones; a.n = n; a.W = row_len; a.pivot = pivot; a.pivot_ptr = nullptr;
-    a.zone_pivots = nullptr;
-    a.has_nodata = has_nodata; a.nodata = nodata;
-    a.keys = (long long *)keys; a.count = (unsigned long long *)count; a.s1 = s1; a.s2 = s2; a.vmin = vmin;
-    a.vmax = vmax; a.cap = cap; a.overflow = overflow; a.sentinel = nullptr;
-    cudaStream_t st = (cudaStream_t)s;
-    int rc;
-#define XRS_ZH(VT)                                                               \
-    switch (zones_dtype) {                                                       \
-        case XRS_I32: rc = launch_zh<VT, int>(a, st); break;                     \
-        case XRS_I64: rc = launch_zh<VT, long long>(a, st); break;               \
-        case XRS_F32: rc = launch_zh<VT, float>(a, st); break;                   \
-        default: rc = launch_zh<VT, double>(a, st); break;                       \
-    }
-    if (values_dtype == XRS_F32) { XRS_ZH(float) } else { XRS_ZH(double) }
-#undef XRS_ZH
-    return rc;
-}
-
 int xrs_zonal_hash_run(const void *values, int values_dtype, const void *zones, int zones_dtype, int64_t n,
                        int64_t row_len, int has_nodata, double nodata, int use_pivot_hint, double pivot_hint,
                        int64_t *keys, int64_t *count, double *s1, double *s2, double *vmin, double *vmax, int cap,
                        double *packed, int max_out, int *flags, xrs_stream_t s) {
-    XRS_REQUIRE(values && zones && keys && count && s1 && s2 && vmin && vmax && packed && flags, "NULL pointer");
-    XRS_REQUIRE(values_dtype == XRS_F32 || values_dtype == XRS_F64, "values must be float32 or float64");
-    XRS_REQUIRE(zones_dtype >= XRS_F32 && zones_dtype <= XRS_I64, "unknown zones dtype");
-    XRS_REQUIRE(cap >= 1024 && (cap & (cap - 1)) == 0, "cap must be a power of two >= 1024");
-    XRS_REQUIRE(max_out >= 1, "max_out must be positive");
-    XRS_REQUIRE(n >= 1 && row_len >= 1 && n % row_len == 0, "n must be a positive multiple of row_len");
-    cudaStream_t st = (cudaStream_t)s;
-    double *pivot_dev = packed + 2;   // the header's pivot cell doubles as the device-side pivot
-    zonal_flags_kernel<<<1, 1, 0, st>>>(flags, pivot_dev, pivot_hint);
-    if (!use_pivot_hint) {
-        if (values_dtype == XRS_F32) zonal_pivot_kernel<float><<<1, 256, 0, st>>>((const float *)values, n, pivot_dev);
-        else zonal_pivot_kernel<double><<<1, 256, 0, st>>>((const double *)values, n, pivot_dev);
-    }
-    zonal_hash_init_kernel<<<(cap + 255) / 256, 256, 0, st>>>((long long *)keys, (unsigned long long *)count, s1, s2,
-                                                             vmin, vmax, cap, flags);
-    XRS_CUDA(cudaGetLastError());
-    ZhArgs a;
-    a.values = values; a.zones = zones; a.n = n; a.W = row_len; a.pivot = 0.0; a.pivot_ptr = pivot_dev;
-    a.zone_pivots = nullptr;
-    a.has_nodata = has_nodata; a.nodata = nodata;
-    a.keys = (long long *)keys; a.count = (unsigned long long *)count; a.s1 = s1; a.s2 = s2; a.vmin = vmin;
-    a.vmax = vmax; a.cap = cap; a.overflow = flags; a.sentinel = flags + 2;
-    int rc;
-#define XRS_ZH(VT)                                                               \
-    switch (zones_dtype) {                                                       \
-        case XRS_I32: rc = launch_zh<VT, int>(a, st); break;                     \
-        case XRS_I64: rc = launch_zh<VT, long long>(a, st); break;               \
-        case XRS_F32: rc = launch_zh<VT, float>(a, st); break;                   \
-        default: rc = launch_zh<VT, double>(a, st); break;                       \
-    }
-    if (values_dtype == XRS_F32) { XRS_ZH(float) } else { XRS_ZH(double) }
-#undef XRS_ZH
-    if (rc != XRS_OK) return rc;
-    zonal_compact_kernel<<<(cap + 255) / 256, 256, 0, st>>>((const long long *)keys, (const unsigned long long *)count,
-                                                           s1, s2, vmin, vmax, cap, packed, max_out, flags);
-    zonal_header_kernel<<<1, 1, 0, st>>>(packed, flags, pivot_dev);
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    return zh_pass(false, values, values_dtype, zones, zones_dtype, n, row_len, has_nodata, nodata, use_pivot_hint,
+                   pivot_hint, nullptr, keys, count, s1, s2, vmin, vmax, cap, packed, max_out, flags, (cudaStream_t)s);
 }
 
 int xrs_zonal_hash_second_pass(const void *values, int values_dtype, const void *zones, int zones_dtype, int64_t n,
                                int64_t row_len, int has_nodata, double nodata, const int64_t *keys,
                                const double *zone_pivots, int64_t *count, double *s1, double *s2, double *vmin,
                                double *vmax, int cap, double *packed, int max_out, int *flags, xrs_stream_t s) {
-    XRS_REQUIRE(values && zones && keys && zone_pivots && count && s1 && s2 && vmin && vmax && packed && flags,
-                "NULL pointer");
-    XRS_REQUIRE(values_dtype == XRS_F32 || values_dtype == XRS_F64, "values must be float32 or float64");
-    XRS_REQUIRE(zones_dtype >= XRS_F32 && zones_dtype <= XRS_I64, "unknown zones dtype");
-    XRS_REQUIRE(cap >= 1024 && (cap & (cap - 1)) == 0, "cap must be a power of two >= 1024");
-    XRS_REQUIRE(max_out >= 1, "max_out must be positive");
-    XRS_REQUIRE(n >= 1 && row_len >= 1 && n % row_len == 0, "n must be a positive multiple of row_len");
-    cudaStream_t st = (cudaStream_t)s;
-    double *pivot_dev = packed + 2;
-    zonal_flags_kernel<<<1, 1, 0, st>>>(flags, pivot_dev, 0.0);
-    zonal_hash_reset_kernel<<<(cap + 255) / 256, 256, 0, st>>>((unsigned long long *)count, s1, s2, vmin, vmax, cap);
-    XRS_CUDA(cudaGetLastError());
-    ZhArgs a;
-    a.values = values; a.zones = zones; a.n = n; a.W = row_len; a.pivot = 0.0; a.pivot_ptr = nullptr;
-    a.zone_pivots = zone_pivots;
-    a.has_nodata = has_nodata; a.nodata = nodata;
-    a.keys = (long long *)keys;   // every key of this raster is already in the table: find-or-insert only finds
-    a.count = (unsigned long long *)count; a.s1 = s1; a.s2 = s2; a.vmin = vmin; a.vmax = vmax; a.cap = cap;
-    a.overflow = flags; a.sentinel = nullptr;
-    int rc;
-#define XRS_ZH(VT)                                                               \
-    switch (zones_dtype) {                                                       \
-        case XRS_I32: rc = launch_zh<VT, int, true>(a, st); break;               \
-        case XRS_I64: rc = launch_zh<VT, long long, true>(a, st); break;         \
-        case XRS_F32: rc = launch_zh<VT, float, true>(a, st); break;             \
-        default: rc = launch_zh<VT, double, true>(a, st); break;                 \
-    }
-    if (values_dtype == XRS_F32) { XRS_ZH(float) } else { XRS_ZH(double) }
-#undef XRS_ZH
-    if (rc != XRS_OK) return rc;
-    zonal_compact_kernel<<<(cap + 255) / 256, 256, 0, st>>>((const long long *)keys, (const unsigned long long *)count,
-                                                           s1, s2, vmin, vmax, cap, packed, max_out, flags);
-    zonal_header_kernel<<<1, 1, 0, st>>>(packed, flags, pivot_dev);
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    // every key of this raster is already in the table: the kernel's find-or-insert only finds
+    return zh_pass(true, values, values_dtype, zones, zones_dtype, n, row_len, has_nodata, nodata, 1, 0.0,
+                   zone_pivots, (int64_t *)keys, count, s1, s2, vmin, vmax, cap, packed, max_out, flags,
+                   (cudaStream_t)s);
 }
 
 int xrs_zonal_pair_count(const float *values, const int32_t *zones, int64_t n, int64_t row_len, int has_nodata,
                          double nodata, int64_t *keys, int64_t *count, int cap, int *overflow, xrs_stream_t s) {
-    if (n <= 0) return XRS_OK;
-    XRS_REQUIRE(values && zones && keys && count && overflow, "NULL pointer");
+    XRS_REQUIRE(keys && count && overflow, "NULL pointer");
     XRS_REQUIRE(cap >= 1024 && (cap & (cap - 1)) == 0, "cap must be a power of two >= 1024");
+    cudaStream_t st = (cudaStream_t)s;
+    // the table is emptied also for an empty raster: the caller reads its keys back
+    zonal_table_init_kernel<<<(cap + 255) / 256, 256, 0, st>>>((long long *)keys, (unsigned long long *)count, nullptr,
+                                                               nullptr, nullptr, nullptr, cap);
+    XRS_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
+    if (n <= 0) return XRS_OK;
+    XRS_REQUIRE(values && zones, "NULL pointer");
     XRS_REQUIRE(row_len >= 1 && n % row_len == 0, "n must be a multiple of row_len");
     ZpArgs a;
     a.values = values; a.zones = (const int *)zones; a.n = n; a.W = row_len; a.has_nodata = has_nodata;
     a.nodata = (float)nodata; a.keys = (long long *)keys; a.count = (unsigned long long *)count; a.cap = cap;
     a.overflow = overflow;
-    const int64_t n_tasks = ((row_len + 127) / 128) * ((n / row_len + kZhSegRows - 1) / kZhSegRows);
-    int64_t grid = (int64_t)sm_count() * 4;
-    const int64_t need = (n_tasks + kZhThreads / 32 - 1) / (kZhThreads / 32);
-    if (grid > need) grid = need;
-    if (grid < 1) grid = 1;
-    zonal_pair_kernel<<<(unsigned)grid, kZhThreads, 0, (cudaStream_t)s>>>(a);
-    XRS_CUDA(cudaGetLastError());
-    return XRS_OK;
+    const int64_t grid = std::max<int64_t>(1, std::min((int64_t)sm_count() * 4, zh_ctas_for_tasks(n, row_len)));
+    return launch(zonal_pair_kernel, grid, kZhThreads, 0, st, kZonalPair, a);
 }
 
 }  // extern "C"

@@ -1,6 +1,6 @@
 """xrspatial.zonal.stats on the CUDA backend (reference: zonal.py:422-667).
 
-One streaming pass (xrs_zonal_hash_accumulate) discovers the zone ids and produces per-zone count /
+One streaming pass (xrs_zonal_hash_run) discovers the zone ids and produces per-zone count /
 sum / sum-of-squares / min / max partials; mean, std (ddof=0) and var are finalised from them in
 float64.  `majority` counts (zone, value) pairs in a second pass (hash table; a device sort when
 the values are too varied for the table).  Custom callables (`stats_funcs` given as a dict, exactly
@@ -19,12 +19,18 @@ from .utils import (ArrayTypeFunctionMapping, as_device_tensor, like_container, 
                     validate_arrays)
 
 _DEFAULT_STATS = ("mean", "max", "min", "sum", "std", "var", "count", "majority")
-_PARTIAL_STATS = ("mean", "max", "min", "sum", "std", "var", "count")
 
 
-def _dtype_code(t):
+def _ptr(t):
+    return ctypes.c_void_p(t.data_ptr())
+
+
+def _device_tensor(a):
+    """A numpy array copied to the current CUDA device; a device array viewed as a torch tensor."""
     import torch
-    return {torch.float32: 0, torch.float64: 1, torch.int32: 2, torch.int64: 3}.get(t.dtype)
+    if isinstance(a, np.ndarray):
+        return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    return as_device_tensor(a)
 
 
 def _prepare(t, allow):
@@ -78,6 +84,46 @@ def _sentinel_partials(zones_t, values_t, nodata_values, pivot):
                 min=np.array([float(vv.min()) if n else np.inf]), max=np.array([float(vv.max()) if n else -np.inf]))
 
 
+def _empty_partials(nz):
+    return dict(count=np.zeros(nz, np.int64), s1=np.zeros(nz), s2=np.zeros(nz), min=np.full(nz, np.inf),
+                max=np.full(nz, -np.inf))
+
+
+def _table_pass(entry, zones_t, values_t, nodata_values, table_args, keys, acc, sentinel_pivot=None):
+    """One pass of the group-by entry point `entry` over the hash table `keys`, accumulating into `acc` (rows count
+    as int64 bit patterns, s1, s2, min, max); `table_args` are the arguments between `nodata` and `count`, tensors
+    passed by pointer.  None when the table overflowed, else (ids, part, pivot): the zones met, in table order;
+    their partials; the shift of the sums.  The zone INT64_MIN, which the table cannot hold, is appended from
+    masked reductions about `sentinel_pivot` (default: the pass's pivot)."""
+    import torch
+    dt = lambda t: _lib.DTYPES[str(t.dtype).replace("torch.", "")]  # noqa: E731
+    packed = torch.empty(_HDR + 6 * _MAX_OUT, dtype=torch.float64, device=values_t.device)
+    flags = torch.empty(3, dtype=torch.int32, device=values_t.device)
+    with torch.cuda.device(values_t.device):
+        _lib.call(entry, _ptr(values_t), dt(values_t), _ptr(zones_t), dt(zones_t), values_t.numel(),
+                  int(values_t.shape[-1]) if values_t.dim() else 1,
+                  0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
+                  *(_ptr(a) if torch.is_tensor(a) else a for a in table_args), *(_ptr(r) for r in acc),
+                  keys.numel(), _ptr(packed), _MAX_OUT, _ptr(flags), stream_ptr(values_t))
+    host = packed.cpu().numpy()                    # the one synchronising copy
+    n_used, overflow, pivot, sentinel = int(host[0]), int(host[1]), float(host[2]), int(host[3])
+    if overflow:
+        return None
+    if n_used <= _MAX_OUT:
+        rows = host[_HDR:].reshape(6, _MAX_OUT)[:, :n_used]
+    else:                                          # many zones: gather the used slots of the table itself
+        used = torch.nonzero(keys != _EMPTY_KEY).reshape(-1)
+        rows = torch.cat([keys[used].view(torch.float64)[None], acc[:, used]]).cpu().numpy()
+    ids = _keys_to_ids(np.ascontiguousarray(rows[0]).view(np.int64), zones_t.dtype)
+    part = dict(count=np.ascontiguousarray(rows[1]).view(np.int64).copy(), s1=rows[2].copy(), s2=rows[3].copy(),
+                min=rows[4].copy(), max=rows[5].copy())
+    if sentinel:
+        ids = np.append(ids, np.int64(_EMPTY_KEY))
+        sp = _sentinel_partials(zones_t, values_t, nodata_values, pivot if sentinel_pivot is None else sentinel_pivot)
+        part = {n: np.append(a, sp[n]) for n, a in part.items()}
+    return ids, part, pivot
+
+
 def hash_partials(zones_t, values_t, nodata_values=None, comm=None, cap=1 << 16, table=None):
     """One streaming pass that discovers the zone ids and accumulates their partials
     (xrs_zonal_hash_run: pivot sampling, table init, accumulation and compaction are enqueued
@@ -90,45 +136,20 @@ def hash_partials(zones_t, values_t, nodata_values=None, comm=None, cap=1 << 16,
     import torch
     dev = values_t.device
     hint = _sample_pivot(values_t, comm) if comm is not None else None
-    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
     if values_t.numel() == 0:
-        zdt = np.float32 if zones_t.dtype == torch.float32 else np.float64 if zones_t.dtype == torch.float64 else \
-            np.int32 if zones_t.dtype == torch.int32 else np.int64
-        e = np.zeros(0)
-        return np.zeros(0, zdt), dict(count=np.zeros(0, np.int64), s1=e, s2=e.copy(), min=e.copy(), max=e.copy()), 0.0
+        return _keys_to_ids(np.zeros(0, np.int64), zones_t.dtype), _empty_partials(0), 0.0
     while True:
         # one blob: rows = keys, count (int64 bit patterns), s1, s2, min, max
         blob = torch.empty((6, cap), dtype=torch.float64, device=dev)
-        packed = torch.empty(_HDR + 6 * _MAX_OUT, dtype=torch.float64, device=dev)
-        flags = torch.empty(3, dtype=torch.int32, device=dev)
-        keys, count = blob[0].view(torch.int64), blob[1].view(torch.int64)
-        with torch.cuda.device(dev):
-            _lib.call("xrs_zonal_hash_run", P(values_t), _dtype_code(values_t), P(zones_t), _dtype_code(zones_t),
-                      values_t.numel(), int(values_t.shape[-1]) if values_t.dim() else 1,
-                      0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
-                      0 if hint is None else 1, 0.0 if hint is None else float(hint),
-                      P(keys), P(count), P(blob[2]), P(blob[3]), P(blob[4]), P(blob[5]), cap,
-                      P(packed), _MAX_OUT, P(flags), stream_ptr(values_t))
-        host = packed.cpu().numpy()                    # the one synchronising copy
-        n_used, overflow, pivot, sentinel = int(host[0]), int(host[1]), float(host[2]), int(host[3])
-        if overflow == 0:
+        keys = blob[0].view(torch.int64)
+        res = _table_pass("xrs_zonal_hash_run", zones_t, values_t, nodata_values,
+                          (0 if hint is None else 1, 0.0 if hint is None else float(hint), keys), keys, blob[1:])
+        if res is not None:
             break
         if cap >= (1 << 24):
             raise NotImplementedError("more than 16M distinct zones are not supported")
         cap *= 16
-    if n_used <= _MAX_OUT:
-        rows = host[_HDR:].reshape(6, _MAX_OUT)[:, :n_used]
-    else:                                               # many zones: gather the used slots of the table itself
-        used = torch.nonzero(keys != _EMPTY_KEY).reshape(-1)
-        rows = blob[:, used].cpu().numpy()
-    k = np.ascontiguousarray(rows[0]).view(np.int64)
-    part = dict(count=np.ascontiguousarray(rows[1]).view(np.int64).copy(), s1=rows[2].copy(), s2=rows[3].copy(),
-                min=rows[4].copy(), max=rows[5].copy())
-    ids = _keys_to_ids(k, zones_t.dtype)
-    if sentinel:
-        ids = np.append(ids, np.int64(_EMPTY_KEY))
-        sp = _sentinel_partials(zones_t, values_t, nodata_values, pivot)
-        part = {n: np.append(a, sp[n]) for n, a in part.items()}
+    ids, part, pivot = res
     if table is not None:
         table.update(keys=keys, cap=cap)
     if comm is not None:
@@ -155,8 +176,7 @@ def second_pass_partials(zones_t, values_t, table, ids, means, nodata_values=Non
     import torch
     dev = values_t.device
     nz = len(ids)
-    part = dict(count=np.zeros(nz, np.int64), s1=np.zeros(nz), s2=np.zeros(nz),
-                min=np.full(nz, np.inf), max=np.full(nz, -np.inf))
+    part = _empty_partials(nz)
     if nz and values_t.numel():
         keys, cap = table["keys"], table["cap"]
         fz = zones_t.dtype.is_floating_point
@@ -165,42 +185,15 @@ def second_pass_partials(zones_t, values_t, table, ids, means, nodata_values=Non
         slot_ids = keys.view(torch.float64) if fz else keys
         idx = torch.searchsorted(ids_t, slot_ids).clamp_(max=nz - 1)
         pivots = means_t[idx].contiguous()                 # empty slots get some zone's mean: never read
-        blob = torch.empty((5, cap), dtype=torch.float64, device=dev)
-        packed = torch.empty(_HDR + 6 * _MAX_OUT, dtype=torch.float64, device=dev)
-        flags = torch.empty(3, dtype=torch.int32, device=dev)
-        count = blob[0].view(torch.int64)
-        P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
-        with torch.cuda.device(dev):
-            _lib.call("xrs_zonal_hash_second_pass", P(values_t), _dtype_code(values_t), P(zones_t),
-                      _dtype_code(zones_t), values_t.numel(), int(values_t.shape[-1]) if values_t.dim() else 1,
-                      0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
-                      P(keys), P(pivots), P(count), P(blob[1]), P(blob[2]), P(blob[3]), P(blob[4]), cap,
-                      P(packed), _MAX_OUT, P(flags), stream_ptr(values_t))
-        host = packed.cpu().numpy()
-        n_used = int(host[0])
-        if n_used <= _MAX_OUT:
-            rows = host[_HDR:].reshape(6, _MAX_OUT)[:, :n_used]
-        else:
-            used = torch.nonzero(keys != _EMPTY_KEY).reshape(-1)
-            rows = torch.cat([keys[used].view(torch.float64)[None], blob[:, used]]).cpu().numpy()
-        local = _keys_to_ids(np.ascontiguousarray(rows[0]).view(np.int64), zones_t.dtype)
+        acc = torch.empty((5, cap), dtype=torch.float64, device=dev)
+        # sorted ids: the INT64_MIN zone, when present, comes first
+        local, lpart, _ = _table_pass("xrs_zonal_hash_second_pass", zones_t, values_t, nodata_values, (keys, pivots),
+                                      keys, acc, sentinel_pivot=float(means[0]))
         pos = np.searchsorted(ids, local)
-        part["count"][pos] = np.ascontiguousarray(rows[1]).view(np.int64)
-        for i, n in enumerate(("s1", "s2", "min", "max")):
-            part[n][pos] = rows[2 + i]
-        if not fz and ids[0] == _EMPTY_KEY:            # sorted ids: the INT64_MIN zone comes first
-            sp = _sentinel_partials(zones_t, values_t, nodata_values, float(means[0]))
-            for n in part:
-                part[n][0] = sp[n][0]
+        for n in part:
+            part[n][pos] = lpart[n]
     if comm is not None and nz:
-        import torch.distributed as dist
-        t = {n: torch.as_tensor(a, device=dev) for n, a in part.items()}
-        dist.all_reduce(t["count"], op=dist.ReduceOp.SUM, group=comm)
-        dist.all_reduce(t["s1"], op=dist.ReduceOp.SUM, group=comm)
-        dist.all_reduce(t["s2"], op=dist.ReduceOp.SUM, group=comm)
-        dist.all_reduce(t["min"], op=dist.ReduceOp.MIN, group=comm)
-        dist.all_reduce(t["max"], op=dist.ReduceOp.MAX, group=comm)
-        part = {n: v.cpu().numpy() for n, v in t.items()}
+        part = _allreduce_partials(part, dev, comm)
     return part
 
 
@@ -213,43 +206,59 @@ class _PairTableOverflow(Exception):
     """more distinct (zone, value) pairs than the hash table is allowed to grow to"""
 
 
-def pair_counts(zones_t, values_t, nodata_values=None, comm=None, cap=1 << 20, max_cap=1 << 26):
-    """(zone ids int64, values float64, counts int64) of every distinct valid (zone, value) pair:
-    one pass of xrs_zonal_pair_count over (int32 zone, float32 value) pairs."""
+_PAIR_CAP = 1 << 20               # first size of the pair table
+_PAIR_MAX_CAP = 1 << 26           # crosstab lets it grow to this (1 GiB of keys and counts)
+_MAJORITY_PAIR_MAX_CAP = 1 << 24  # majority grows it no further and groups by one device sort instead
+
+
+def _float32_exact(values_t):
+    """`values_t` as float32, or None when a finite value is not exact in float32.  float32 rasters are used in
+    place: the pair kernel itself folds -0.0 into 0.0, and a `+ 0.0` copy cost a full read + write of the raster."""
     import torch
-    dev = values_t.device
-    if zones_t.dtype != torch.int32:
-        if zones_t.dtype.is_floating_point:
-            zi = zones_t.to(torch.int32)
-            if not bool((zi.to(zones_t.dtype) == zones_t)[torch.isfinite(zones_t)].all()):
-                raise NotImplementedError("'majority' needs integer-valued zone ids")
-        else:
-            zi = zones_t.to(torch.int32)
-            if not bool((zi.to(zones_t.dtype) == zones_t).all()):
-                raise NotImplementedError("'majority' needs zone ids that fit in int32")
-        finite_zone = torch.isfinite(zones_t) if zones_t.dtype.is_floating_point else None
-    else:
-        zi, finite_zone = zones_t, None
-    # float32 rasters are read in place (the kernel itself folds -0.0 into 0.0, one value for np.unique):
-    # a `+ 0.0` copy here cost a full extra read + write of the raster
-    vf = values_t if values_t.dtype == torch.float32 else values_t.to(torch.float32)
-    if values_t.dtype != torch.float32 and not bool(((vf.to(values_t.dtype) == values_t) | ~torch.isfinite(values_t)).all()):
+    if values_t.dtype == torch.float32:
+        return values_t
+    vf = values_t.to(torch.float32)
+    return vf if bool(((vf.to(values_t.dtype) == values_t) | ~torch.isfinite(values_t)).all()) else None
+
+
+def _pair_inputs(zones_t, values_t):
+    """The int32 zones and float32 values of the (zone, value) pair table; NotImplementedError when the
+    narrowing would not be exact.  Cells whose float zone id is not finite get NaN values, so they drop out."""
+    import torch
+    zi = zones_t if zones_t.dtype == torch.int32 else zones_t.to(torch.int32)
+    if zones_t.dtype.is_floating_point:
+        finite_zone = torch.isfinite(zones_t)
+        if not bool((zi.to(zones_t.dtype) == zones_t)[finite_zone].all()):
+            raise NotImplementedError("'majority' needs integer-valued zone ids")
+    elif zi is not zones_t and not bool((zi.to(zones_t.dtype) == zones_t).all()):
+        raise NotImplementedError("'majority' needs zone ids that fit in int32")
+    vf = _float32_exact(values_t)
+    if vf is None:
         raise NotImplementedError("'majority' needs values that are exact in float32")
-    if finite_zone is not None:
-        vf = torch.where(finite_zone, vf, torch.full_like(vf, float("nan")))  # cells of NaN zones drop out
-    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    if zones_t.dtype.is_floating_point:
+        vf = torch.where(finite_zone, vf, torch.full_like(vf, float("nan")))
+    return zi, vf
+
+
+def pair_counts(zones_t, values_t, nodata_values=None, comm=None, cap=None, max_cap=None):
+    """(zone ids int64, values float64, counts int64) of every distinct valid (zone, value) pair:
+    one pass of xrs_zonal_pair_count over int32 zones and float32 values.  The table starts at `cap` slots
+    (default _PAIR_CAP) and grows up to `max_cap` (default _PAIR_MAX_CAP), then raises _PairTableOverflow."""
+    import torch
+    if zones_t.dtype != torch.int32 or values_t.dtype != torch.float32:
+        raise TypeError("pair_counts takes int32 zones and float32 values")
+    cap = _PAIR_CAP if cap is None else cap
+    max_cap = _PAIR_MAX_CAP if max_cap is None else max_cap
+    dev = values_t.device
+    vf, zi = values_t.contiguous(), zones_t.contiguous()
     while True:
         keys = torch.empty(cap, dtype=torch.int64, device=dev)
         count = torch.empty(cap, dtype=torch.int64, device=dev)
-        dummy = torch.empty((4, cap), dtype=torch.float64, device=dev)
         ovf = torch.empty(1, dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
-            st = stream_ptr(vf)
-            _lib.call("xrs_zonal_hash_init", P(keys), P(count), P(dummy[0]), P(dummy[1]), P(dummy[2]), P(dummy[3]),
-                      cap, P(ovf), st)
-            _lib.call("xrs_zonal_pair_count", P(vf.contiguous()), P(zi.contiguous()), vf.numel(),
-                      int(vf.shape[-1]) if vf.dim() else 1, 0 if nodata_values is None else 1,
-                      0.0 if nodata_values is None else float(nodata_values), P(keys), P(count), cap, P(ovf), st)
+            _lib.call("xrs_zonal_pair_count", _ptr(vf), _ptr(zi), vf.numel(), int(vf.shape[-1]) if vf.dim() else 1,
+                      0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
+                      _ptr(keys), _ptr(count), cap, _ptr(ovf), stream_ptr(vf))
         if int(ovf.item()) == 0:
             break
         if cap >= max_cap:
@@ -327,12 +336,10 @@ def majority_by_zone(zones_t, values_t, unique_zones, nodata_values=None, comm=N
     out = np.full(len(uz), np.nan)
     if len(uz) == 0:
         return out
-    vf = values_t.to(torch.float32)
-    exact32 = values_t.dtype == torch.float32 or \
-        bool(((vf.to(values_t.dtype) == values_t) | ~torch.isfinite(values_t)).all())
-    if zones_t.dtype == torch.int32 and exact32:
+    vf = _float32_exact(values_t)
+    if zones_t.dtype == torch.int32 and vf is not None:
         try:
-            zone, val, c = pair_counts(zones_t, values_t, nodata_values, comm, max_cap=1 << 24)
+            zone, val, c = pair_counts(zones_t, vf, nodata_values, comm, max_cap=_MAJORITY_PAIR_MAX_CAP)
             order = np.lexsort((val, -c, zone))      # per zone: highest count first, then smallest value
             zone, val = zone[order], val[order]
             first = np.r_[True, zone[1:] != zone[:-1]]
@@ -346,7 +353,7 @@ def majority_by_zone(zones_t, values_t, unique_zones, nodata_values=None, comm=N
         raise NotImplementedError("'majority' over row stripes needs int32 zones and categorical float32-exact "
                                   "values (the sort-based path is single-GPU)")
     z = zones_t.reshape(-1)
-    v = (vf if exact32 else values_t.to(torch.float64)).reshape(-1) + 0.0   # -0.0 and 0.0 are one value
+    v = (vf if vf is not None else values_t.to(torch.float64)).reshape(-1) + 0.0   # -0.0 and 0.0 are one value
     ok = torch.isfinite(v)
     if nodata_values is not None:
         ok &= v != float(nodata_values)
@@ -369,6 +376,17 @@ def _zone_index(z, sel):
     return idx, ids_t[idx] == zk      # NaN zones match nothing
 
 
+def _allreduce_partials(part, dev, comm):
+    """Partials of the same zones on every rank combined over `comm`: SUM count / s1 / s2, MIN min, MAX max."""
+    import torch
+    import torch.distributed as dist
+    t = {n: torch.as_tensor(a, device=dev) for n, a in part.items()}
+    for n, op in (("count", dist.ReduceOp.SUM), ("s1", dist.ReduceOp.SUM), ("s2", dist.ReduceOp.SUM),
+                  ("min", dist.ReduceOp.MIN), ("max", dist.ReduceOp.MAX)):
+        dist.all_reduce(t[n], op=op, group=comm)
+    return {n: v.cpu().numpy() for n, v in t.items()}
+
+
 def allreduce_tables(ids, part, dev, comm):
     """Combine the per-stripe tables of all ranks: the id lists are all-gathered (a few KB), every
     rank scatters its partials into dense arrays over the sorted union of ids, and the dense
@@ -387,23 +405,12 @@ def allreduce_tables(ids, part, dev, comm):
     dist.all_gather(gathered, mine, group=comm)
     union = np.unique(np.concatenate([g[:int(c.item())].cpu().numpy() for g, c in zip(gathered, counts)]))
     pos = np.searchsorted(union, np.asarray(ids, dtype=np.float64))
-    nz = len(union)
-    dense = dict(count=torch.zeros(nz, dtype=torch.int64, device=dev),
-                 s1=torch.zeros(nz, dtype=torch.float64, device=dev),
-                 s2=torch.zeros(nz, dtype=torch.float64, device=dev),
-                 min=torch.full((nz,), float("inf"), dtype=torch.float64, device=dev),
-                 max=torch.full((nz,), float("-inf"), dtype=torch.float64, device=dev))
-    if len(ids):
-        idx = torch.as_tensor(pos, device=dev)
-        for k in dense:
-            dense[k][idx] = torch.as_tensor(part[k], device=dev)
-    if nz:
-        dist.all_reduce(dense["count"], op=dist.ReduceOp.SUM, group=comm)
-        dist.all_reduce(dense["s1"], op=dist.ReduceOp.SUM, group=comm)
-        dist.all_reduce(dense["s2"], op=dist.ReduceOp.SUM, group=comm)
-        dist.all_reduce(dense["min"], op=dist.ReduceOp.MIN, group=comm)
-        dist.all_reduce(dense["max"], op=dist.ReduceOp.MAX, group=comm)
-    return union.astype(np.asarray(ids).dtype), {k: v.cpu().numpy() for k, v in dense.items()}
+    dense = _empty_partials(len(union))
+    for k in dense:
+        dense[k][pos] = part[k]
+    if len(union):
+        dense = _allreduce_partials(dense, dev, comm)
+    return union.astype(np.asarray(ids).dtype), dense
 
 
 # Bound on the relative error of the kernel's float64 sums (count, s1, s2 are each a float64 sum over a
@@ -465,6 +472,31 @@ def finalize(part, pivot, stats_funcs):
     return cols
 
 
+def _partial_columns(zt, vt, table, ids, part, pivot, names, nodata_values, comm, pos=None):
+    """finalize(...) of `names` over the zones ids[pos] (all `ids` when pos is None) from hash_partials' results.
+    mean / sum / std / var come from a second pass about each zone's own mean (numpy's two-pass statistics) for
+    float64 rasters when std / var are asked for, and whenever the one-pass sums over these zones may be too
+    inaccurate (zones far from the pivot for their spread)."""
+    import torch
+    sel_part = part if pos is None else {n: a[pos] for n, a in part.items()}
+    sel_pivot = np.full(len(sel_part["count"]), pivot)
+    moments = [s for s in names if s in ("mean", "sum", "std", "var")]
+    second = len(sel_pivot) > 0 and bool(moments) and \
+        ((vt.dtype == torch.float64 and any(s in ("std", "var") for s in names)) or
+         one_pass_inaccurate(sel_part, sel_pivot))
+    cols = finalize(sel_part, sel_pivot, [s for s in names if not (second and s in moments)])
+    if second:
+        cnt = part["count"].astype(np.float64)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            means = np.where(cnt > 0, pivot + part["s1"] / cnt, 0.0)
+        part2 = second_pass_partials(zt, vt, table, ids, means, nodata_values, comm=comm)
+        if pos is not None:
+            part2 = {n: a[pos] for n, a in part2.items()}
+            means = means[pos]
+        cols.update(finalize(part2, means, moments))
+    return cols
+
+
 def _stats_device(zones, values, zone_ids, stats_funcs, nodata_values, return_type='pandas.DataFrame',
                   comm=None):
     """Device runner (replaces zonal.py:335 `_stats_cupy`)."""
@@ -478,35 +510,16 @@ def _stats_device(zones, values, zone_ids, stats_funcs, nodata_values, return_ty
     names = list(stats_funcs)
     table = {}
     unique_zones, part_all, pivot0 = hash_partials(zt, vt, nodata_values, comm=comm, table=table)
-    zdtype = unique_zones.dtype
     if zone_ids is None:
-        sel = unique_zones
-        part = part_all
+        sel, pos = unique_zones, None
     else:
-        sel = np.array([z for z in np.unique(zone_ids) if z in unique_zones], dtype=zdtype)
+        sel = np.array([z for z in np.unique(zone_ids) if z in unique_zones], dtype=unique_zones.dtype)
         pos = np.searchsorted(unique_zones, sel)
-        part = {n: a[pos] for n, a in part_all.items()}
-    pivot = np.full(len(sel), pivot0)
-    # mean / sum / std / var come from a second pass about each zone's own mean (numpy's two-pass
-    # statistics) for float64 rasters when std / var are asked for, and for float32 rasters when the
-    # one-pass sums about the global pivot may be too inaccurate (zones far from the pivot for their spread)
-    sv = [s for s in names if s in ("std", "var")]
-    moments = [s for s in names if s in ("mean", "sum", "std", "var")]
-    second = len(sel) > 0 and bool(moments) and \
-        ((vt.dtype == torch.float64 and bool(sv)) or one_pass_inaccurate(part, pivot))
-    cols = finalize(part, pivot, [s for s in names if s != "majority" and not (second and s in moments)])
+    cols = _partial_columns(zt, vt, table, unique_zones, part_all, pivot0, [s for s in names if s != "majority"],
+                            nodata_values, comm, pos)
     if "majority" in names:
         maj = majority_by_zone(zt, vt, unique_zones, nodata_values, comm=comm)
-        cols["majority"] = maj if zone_ids is None else maj[pos]
-    if second:
-        cnt = part_all["count"].astype(np.float64)
-        with np.errstate(invalid="ignore", divide="ignore"):
-            means = np.where(cnt > 0, pivot0 + part_all["s1"] / cnt, 0.0)
-        part2 = second_pass_partials(zt, vt, table, unique_zones, means, nodata_values, comm=comm)
-        if zone_ids is not None:
-            part2 = {n: a[pos] for n, a in part2.items()}
-            means = means[pos]
-        cols.update(finalize(part2, means, moments))
+        cols["majority"] = maj if pos is None else maj[pos]
     if return_type == 'pandas.DataFrame':
         d = {"zone": sel}
         for s in names:
@@ -585,9 +598,7 @@ def _stats_custom(zones, values, zone_ids, stats_funcs, nodata_values, return_ty
 
 def _stats_host(zones, values, zone_ids, stats_funcs, nodata_values, return_type='pandas.DataFrame'):
     """numpy runner (replaces zonal.py:280 `_stats_numpy`): upload, same device pass."""
-    import torch
-    zt = torch.from_numpy(np.ascontiguousarray(zones)).cuda()
-    vt = torch.from_numpy(np.ascontiguousarray(values)).cuda()
+    zt, vt = _device_tensor(zones), _device_tensor(values)
     if isinstance(stats_funcs, dict):
         res = _stats_custom(zt, vt, zone_ids, stats_funcs, nodata_values, return_type, host=True)
     else:
@@ -712,11 +723,8 @@ def _crosstab_3d(zones, values, zone_ids, cat_ids, layer, agg, nodata_values, co
     except (IndexError, KeyError, TypeError):
         raise ValueError("Invalid `layer`")
     axis = list(values.dims).index(ldim)
-    host = isinstance(values.data, np.ndarray)
-    vt = torch.from_numpy(np.ascontiguousarray(values.data)).cuda() if host else as_device_tensor(values.data)
-    zt = torch.from_numpy(np.ascontiguousarray(zones.data)).cuda() if isinstance(zones.data, np.ndarray) \
-        else as_device_tensor(zones.data)
-    vt = torch.movedim(vt, axis, 0)
+    vt = torch.movedim(_device_tensor(values.data), axis, 0)
+    zt = _device_tensor(zones.data)
     if tuple(zt.shape) != tuple(vt.shape[1:]):
         raise ValueError("Incompatible shapes")
     zt = _prepare(zt, (torch.int32, torch.int64, torch.float32, torch.float64))
@@ -743,15 +751,8 @@ def _crosstab_3d(zones, values, zone_ids, cat_ids, layer, agg, nodata_values, co
         hit = (ids[pos] == sel) if len(ids) else np.zeros(len(sel), bool)
         if agg == "majority":
             col_all = majority_by_zone(zt, lt, ids, nodata_values, comm=comm)
-        elif agg in ("mean", "sum", "std", "var") and len(ids) and \
-                ((lt.dtype == torch.float64 and agg in ("std", "var")) or one_pass_inaccurate(part, pivot0)):
-            cnt = part["count"].astype(np.float64)
-            with np.errstate(invalid="ignore", divide="ignore"):
-                means = np.where(cnt > 0, pivot0 + part["s1"] / cnt, 0.0)
-            part2 = second_pass_partials(zt, lt, table, ids, means, nodata_values, comm=comm)
-            col_all = finalize(part2, means, [agg])[agg]
         else:
-            col_all = finalize(part, np.full(len(ids), pivot0), [agg])[agg]
+            col_all = _partial_columns(zt, lt, table, ids, part, pivot0, [agg], nodata_values, comm)[agg]
         col = np.where(hit, col_all[pos] if len(ids) else np.nan, np.nan)
         if agg == "count":          # np.ma.count of an empty selection is 0, and the column is integer
             col = np.where(np.isnan(col), 0, col).astype(np.int64)
@@ -778,16 +779,13 @@ def crosstab(zones, values, zone_ids=None, cat_ids=None, layer=None, agg="count"
     if agg not in ("percentage", "count"):
         raise ValueError("`agg` method for 2D data array must be one of following ['percentage', 'count']")
     import torch
-    if isinstance(values.data, np.ndarray):
-        zt = torch.from_numpy(np.ascontiguousarray(zones.data)).cuda()
-        vt = torch.from_numpy(np.ascontiguousarray(values.data)).cuda()
-    else:
-        zt, vt = as_device_tensor(zones.data), as_device_tensor(values.data)
+    zt, vt = _device_tensor(zones.data), _device_tensor(values.data)
     zt = _prepare(zt, (torch.int32, torch.int64, torch.float32, torch.float64))
     vt_f = vt.contiguous() if vt.dtype in (torch.float32, torch.float64) else vt.to(torch.float64)
     unique_zones, _, _ = hash_partials(zt, vt_f, None, comm=comm)
+    zi, vf = _pair_inputs(zt, vt_f)
     try:
-        pz, pv, pc = pair_counts(zt, vt_f, nodata_values, comm=comm)
+        pz, pv, pc = pair_counts(zi, vf, nodata_values, comm=comm)
     except _PairTableOverflow:
         raise NotImplementedError("crosstab: more than 64M distinct (zone, category) pairs")
     vdtype = np.dtype(str(vt.dtype).replace("torch.", "")) if not isinstance(values.data, np.ndarray) else values.data.dtype
