@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define XRS_ABI_VERSION 2
+#define XRS_ABI_VERSION 3
 
 typedef void *xrs_stream_t; /* cudaStream_t */
 
@@ -222,35 +222,28 @@ int xrs_zonal_pair_count(const float *values, const int32_t *zones, int64_t n, i
                          int *overflow, xrs_stream_t s);
 
 /* ------------------------------------------------------------------ host-buffer (end-to-end)
- * Same operators on HOST rasters: the library stripes the raster over rows, and overlaps
+ * Same operators on HOST rasters: the library cuts the raster into row chunks and overlaps
  * host->device copies, kernels and device->host copies on internal streams.  `op` selects
- * the operator; scalar parameters are passed in p[0..7] in the order of the device entry
- * point (e.g. slope: p[0]=cellsize_x, p[1]=cellsize_y).  aux/naux carry the excludes
- * (focal mean) or the kernel followed by kh,kw in p[0],p[1] (convolve / focal stat). */
+ * the operator (values 0-3 are also the `op` of xrs_surface_typed). */
 enum xrs_op {
     XRS_OP_SLOPE = 0, XRS_OP_ASPECT = 1, XRS_OP_CURVATURE = 2, XRS_OP_HILLSHADE = 3,
-    XRS_OP_FOCAL_MEAN = 4, XRS_OP_CONVOLVE = 5, XRS_OP_FOCAL_STAT = 6,
-    XRS_OP_FOCAL_MEAN_F64 = 7,     /* in/out are double */
-    XRS_OP_FOCAL_MEAN_F32_F64 = 8  /* in float, out double */
+    XRS_OP_FOCAL_MEAN = 4, XRS_OP_CONVOLVE = 5, XRS_OP_FOCAL_STAT = 6
 };
-/* in/out: float32 rasters (see the two FOCAL_MEAN_F* ops for float64), contiguous rows.
+/* in: H x W cells of `in_dtype`, out: H x W cells, both contiguous rows in host memory:
+ *   slope, aspect, curvature, hillshade: float32 in, or int16 / uint16 / int32 / float64 when
+ *     W % 4 == 0 (xrs_surface_typed behind the pipeline: the raw cells cross PCIe); float32 out.
+ *   focal mean: float32 or float64 in; float64 out (focal.py:257 `astype(float)`).
+ *   convolve, focal stat: float32 in, float32 out.
  * p: slope {csx, csy}; curvature {cellsize}; hillshade {azimuth, altitude};
- *    convolve {kh, kw}; focal stat {kh, kw, stat}.  aux: excludes / kernel (host). */
-int xrs_host_stencil(int op, const void *in, void *out, int64_t H, int64_t W, const double *p,
-                     const double *aux, int naux, int device);
-/* slope / aspect / curvature / hillshade on a HOST raster of int16 / uint16 / int32 / float64 cells
- * (xrs_surface_typed behind the same pipeline; needs W % 4 == 0): the raw cells cross PCIe. */
-int xrs_host_surface_typed(int op, const void *in, int in_dtype, float *out, int64_t H, int64_t W,
-                           const double *p, int device);
-/* The same two entry points over SEVERAL devices: output rows are cut into one stripe per listed
+ *    convolve {kh, kw}; focal stat {kh, kw, stat}.  aux/naux (host): the excludes of focal mean,
+ *    or the kernel of convolve / focal stat.
+ * devices: CUDA ordinals, each at most once.  The output rows are cut into one stripe per listed
  * device, each stripe runs the chunk pipeline on its own host thread and PCIe link; the halo rows
  * of a stripe come from the host raster, so there is no device-to-device traffic.  This is the
  * reference's dask.map_overlap(depth=r, boundary=nan) over row blocks (slope.py:94-97,
- * focal.py:72-75) for host rasters.  devices: CUDA ordinals, each at most once. */
-int xrs_host_stencil_multi(int op, const void *in, void *out, int64_t H, int64_t W, const double *p,
-                           const double *aux, int naux, const int *devices, int n_devices);
-int xrs_host_surface_typed_multi(int op, const void *in, int in_dtype, float *out, int64_t H, int64_t W,
-                                 const double *p, const int *devices, int n_devices);
+ * focal.py:72-75) for host rasters.  A bad request returns XRS_EINVAL before any CUDA call. */
+int xrs_host_stencil(int op, const void *in, int in_dtype, void *out, int64_t H, int64_t W,
+                     const double *p, const double *aux, int naux, const int *devices, int n_devices);
 /* frees the per-device staging buffers the host path keeps between calls */
 int xrs_host_release(int device);
 /* pinned host memory helpers (cudaHostAlloc / cudaFreeHost) for callers that want

@@ -25,12 +25,12 @@ def test_header_declares_the_hot_path():
         assert s in syms
 
 
-def test_library_exports_every_declared_symbol_at_abi_version_2():
+def test_library_exports_every_declared_symbol_at_abi_version_3():
     import xrspatial_b200
     lib = xrspatial_b200._lib.lib()
     for s in header_symbols():
         assert hasattr(lib, s), "libxrs_b200.so does not export %s" % s
-    assert lib.xrs_abi_version() == 2
+    assert lib.xrs_abi_version() == 3
 
 
 def test_ctypes_prototypes_cover_the_header():
@@ -67,3 +67,32 @@ def test_argument_errors_do_not_need_a_gpu():
     assert rc == -1
     with pytest.raises(ValueError):
         xrspatial_b200._lib.check(rc)
+
+
+def test_host_stencil_rejects_bad_requests_before_any_cuda_call():
+    """Every check of xrs_host_stencil runs before its first CUDA call: XRS_EINVAL (not XRS_ECUDA) and
+    a message, also on a machine without a GPU."""
+    import xrspatial_b200
+    _lib = xrspatial_b200._lib
+    lib = _lib.lib()
+    F32, F64, I16 = _lib.DTYPES["float32"], _lib.DTYPES["float64"], _lib.DTYPES["int16"]
+    OPS = _lib.OPS
+    buf = (ctypes.c_double * (64 * 8))()
+    ptr = ctypes.cast(buf, ctypes.c_void_p)
+    p = (ctypes.c_double * 3)(3, 3, 0)
+    k = (ctypes.c_double * 9)(*[1.0] * 9)
+
+    def run(op, in_dtype, H=64, W=8, out=ptr, devices=(0,)):
+        devs = (ctypes.c_int * len(devices))(*devices)
+        return lib.xrs_host_stencil(op, ptr, in_dtype, out, H, W, p, k, 9, devs, len(devices))
+
+    for args, kw, words in (((7, F32), {}, b"unknown op"),
+                            ((8, F32), {}, b"unknown op"),
+                            ((OPS["focal_mean"], I16), {}, b"focal mean"),
+                            ((OPS["convolve"], F64), {}, b"convolve"),
+                            ((OPS["slope"], I16), dict(W=6), b"W % 4"),
+                            ((OPS["slope"], F32), dict(devices=(0, 0)), b"twice"),
+                            ((OPS["slope"], F32), dict(out=None), b"NULL")):
+        assert run(*args, **kw) == _lib.XRS_EINVAL, (args, kw)
+        assert words in lib.xrs_last_error_string(), (args, kw, lib.xrs_last_error_string())
+    assert run(OPS["slope"], F32, H=0) == _lib.XRS_OK

@@ -971,8 +971,8 @@ def test_pinned_cache_is_bounded_and_lru(xb):
 
 
 def test_host_path_over_several_devices_matches_one_device(xb, monkeypatch):
-    """xrs_host_stencil_multi: row stripes over the visible GPUs, halos from the host raster: the
-    result is the single-device result bit for bit (with one GPU the stripes collapse to one)."""
+    """xrs_host_stencil over a list of devices: row stripes over the visible GPUs, halos from the host
+    raster: the result is the single-device result bit for bit (with one GPU the stripes collapse to one)."""
     rng = np.random.default_rng(77)
     z = terrain(rng, 1500, 1024, nans=0.003)
     kern = rng.standard_normal((9, 9))

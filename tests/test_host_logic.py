@@ -378,3 +378,27 @@ def test_row_segments_are_wave_balanced():
         rows = lib.xrs_debug_pick_seg_rows(32768, n_tiles, 296, 12 * kh, kh - 1, 4, 4)
         assert (rows + kh - 1) % 4 == 0 and rows >= 12 * kh
         assert cost(32768, n_tiles, 296, rows, kh - 1) <= 1.06 * 32768 * n_tiles / 296
+
+
+@pytest.mark.parametrize("op, dtype, W, code, out_dtype", [
+    ("slope", np.int16, 8, "int16", np.float32),       # raw 16-bit cells cross PCIe
+    ("slope", np.int16, 6, "float32", np.float32),     # W % 4 != 0: cast on the host
+    ("slope", np.int64, 8, "float32", np.float32),
+    ("focal_mean", np.float32, 8, "float32", np.float64),
+    ("focal_mean", np.float64, 8, "float64", np.float64),
+    ("focal_mean", np.int32, 8, "float64", np.float64),
+    ("convolve", np.float64, 8, "float32", np.float32),
+])
+def test_host_runner_picks_the_cells_and_result_dtype(monkeypatch, op, dtype, W, code, out_dtype):
+    """run_stencil_host's dtype table: which in_dtype code xrs_host_stencil gets and what the result holds."""
+    from xrspatial_b200 import _hostmem
+    calls = []
+    monkeypatch.setattr(utils._lib, "call", lambda name, *args: calls.append((name, args)))
+    monkeypatch.setattr(_hostmem, "empty", np.empty)
+    monkeypatch.setenv("XRS_B200_DEVICES", "0")
+    out = utils.run_stencil_host(op, np.zeros((5, W), dtype), p=(3, 3, 0), aux=(1.0,) * 9)
+    (name, args), = calls
+    assert name == "xrs_host_stencil"
+    assert args[0] == utils._lib.OPS[op]
+    assert args[2] == utils._lib.DTYPES[code]
+    assert out.dtype == out_dtype and out.shape == (5, W)

@@ -10,8 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.path.join(HERE, "libxrs_b200.so")
 
 XRS_OK, XRS_EINVAL, XRS_ECUDA, XRS_EUNSUPPORTED, XRS_ENOMEM = 0, -1, -2, -3, -4
-OPS = dict(slope=0, aspect=1, curvature=2, hillshade=3, focal_mean=4, convolve=5, focal_stat=6,
-           focal_mean_f64=7, focal_mean_f32_f64=8)
+OPS = dict(slope=0, aspect=1, curvature=2, hillshade=3, focal_mean=4, convolve=5, focal_stat=6)
 STATS = dict(mean=0, sum=1, min=2, max=3, std=4, range=5, var=6)
 DTYPES = dict(float32=0, float64=1, int32=2, int64=3, int16=4, uint16=5)
 
@@ -58,10 +57,7 @@ def _declare(lib):
         "xrs_zonal_hash_run": [P, I, P, I, I64, I64, I, D, I, D, P, P, P, P, P, P, I, P, I, P, P],
         "xrs_zonal_hash_second_pass": [P, I, P, I, I64, I64, I, D, P, P, P, P, P, P, P, I, P, I, P, P],
         "xrs_zonal_pair_count": [P, P, I64, I64, I, D, P, P, I, P, P],
-        "xrs_host_stencil": [I, P, P, I64, I64, P, P, I, I],
-        "xrs_host_surface_typed": [I, P, I, P, I64, I64, P, I],
-        "xrs_host_stencil_multi": [I, P, P, I64, I64, P, P, I, P, I],
-        "xrs_host_surface_typed_multi": [I, P, I, P, I64, I64, P, P, I],
+        "xrs_host_stencil": [I, P, I, P, I64, I64, P, P, I, P, I],
         "xrs_host_release": [I],
         "xrs_host_alloc": [ctypes.POINTER(P), I64],
         "xrs_host_free": [P],

@@ -6,8 +6,7 @@ import numpy as np
 
 from . import _lib
 from ._xr import DataArray, Dataset
-from .utils import (device_f32_2d, get_dataarray_resolution, is_device_array, like_container,
-                    stream_ptr)
+from .utils import device_2d, get_dataarray_resolution, is_device_array, like_container, stream_ptr
 
 
 def surface_suite(agg, azimuth=225, angle_altitude=25, products=("slope", "aspect", "curvature", "hillshade")):
@@ -16,13 +15,12 @@ def surface_suite(agg, azimuth=225, angle_altitude=25, products=("slope", "aspec
     import torch
     data = agg.data
     if isinstance(data, np.ndarray):
-        t = torch.from_numpy(np.ascontiguousarray(data, dtype=np.float32)).cuda()
         back = lambda x: x.cpu().numpy()  # noqa: E731
     elif is_device_array(data):
-        t = device_f32_2d(data)
         back = lambda x: like_container(x, data)  # noqa: E731
     else:
         raise TypeError('Unsupported Array Type: {}'.format(type(data)))
+    t = device_2d(data, torch.float32)
     csx, csy = get_dataarray_resolution(agg)
     H, W = t.shape
     outs = {}

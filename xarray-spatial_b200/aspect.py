@@ -1,13 +1,13 @@
 """xrspatial.aspect on the CUDA backend (reference: aspect.py:274-388, planar)."""
 from ._xr import DataArray
 from .dataset_support import supports_dataset
-from .utils import (Z_UNITS, ArrayTypeFunctionMapping, extract_latlon, run_geodesic, run_surface_device,
-                    run_surface_host)
+from .utils import (Z_UNITS, ArrayTypeFunctionMapping, extract_latlon, run_geodesic, run_stencil_host,
+                    run_surface_device)
 
 
 def _run_numpy(data):
-    """replaces aspect.py:56 `_run_numpy`."""
-    return run_surface_host("aspect", data, ())
+    """Host raster -> xrs_host_stencil(XRS_OP_ASPECT) (replaces aspect.py:56 `_run_numpy`)."""
+    return run_stencil_host("aspect", data)
 
 
 def _run_cupy(data):

@@ -102,8 +102,7 @@ def _convolve_2d_numpy(data, kernel):
 def _convolve_2d_cupy(data, kernel):
     """replaces convolution.py:368 `_convolve_2d_cupy` (device raster)."""
     k = _kernel_f64(kernel)
-    kp = k.ctypes.data_as(ctypes.c_void_p)
-    return run_stencil_device("xrs_convolve2d_f32", data, aux=kp, extra_ints=(k.shape[0], k.shape[1]))
+    return run_stencil_device("xrs_convolve2d_f32", data, k.ctypes.data_as(ctypes.c_void_p), k.shape[0], k.shape[1])
 
 
 def convolve_2d(data, kernel):

@@ -9,9 +9,9 @@
 // correct when they coincide with the real raster edge -- interior halo rows are simply
 // not copied back.  Host buffers may be pageable (works, slower) or pinned (xrs_host_alloc).
 //
-// Several GPUs (xrs_host_stencil_multi): the output rows are cut into one stripe per device and
-// every device runs the pipeline above on its stripe from its own host thread -- one PCIe link
-// each, no device-to-device traffic at all, because a stripe's halo rows come straight from the
+// Several GPUs (the `devices` list of xrs_host_stencil): the output rows are cut into one stripe per
+// device and every device runs the pipeline above on its stripe from its own host thread -- one PCIe
+// link each, no device-to-device traffic at all, because a stripe's halo rows come straight from the
 // host raster like any chunk's.  This is the reference's `dask.map_overlap(depth=r)` over row
 // blocks (slope.py:94-97) with the blocks being PCIe-sized.
 #include <mutex>
@@ -59,9 +59,50 @@ static int ensure_cap(void **p, size_t *cap, size_t need) {
     return XRS_OK;
 }
 
+// The cell sizes and halo of a host request.  host_op_shape is the one place that decides them and
+// checks the request, before any CUDA call:
+//   op                                   in_dtype                                        out
+//   SLOPE, ASPECT, CURVATURE, HILLSHADE  F32; F64, I32, I16, U16 when W % 4 == 0         float32
+//   FOCAL_MEAN                           F32, F64                                        float64
+//   CONVOLVE, FOCAL_STAT                 F32                                             float32
+struct OpShape {
+    int in_size, out_size, radius;
+};
+
+static int host_op_shape(int op, int in_dtype, const double *p, const double *aux, int64_t W, OpShape *sh) {
+    sh->in_size = (in_dtype == XRS_F64) ? 8 : (in_dtype == XRS_I16 || in_dtype == XRS_U16) ? 2 : 4;
+    sh->out_size = 4;
+    sh->radius = 1;
+    switch (op) {
+        case XRS_OP_SLOPE:
+        case XRS_OP_ASPECT:
+        case XRS_OP_CURVATURE:
+        case XRS_OP_HILLSHADE:
+            XRS_REQUIRE(p || op == XRS_OP_ASPECT, "scalar parameters missing");
+            if (in_dtype == XRS_F32) return XRS_OK;
+            // raw cells go to the direct-ingest TMA kernels (xrs_surface_typed), which need W % 4 == 0
+            XRS_REQUIRE(in_dtype == XRS_F64 || in_dtype == XRS_I32 || in_dtype == XRS_I16 || in_dtype == XRS_U16,
+                        "in_dtype must be float32, int16, uint16, int32 or float64");
+            XRS_REQUIRE(W % 4 == 0, "int16 / uint16 / int32 / float64 host input needs W % 4 == 0");
+            return XRS_OK;
+        case XRS_OP_FOCAL_MEAN:  // float64 out: focal.mean's `astype(float)` (focal.py:257)
+            XRS_REQUIRE(in_dtype == XRS_F32 || in_dtype == XRS_F64, "focal mean takes float32 or float64 cells");
+            sh->out_size = 8;
+            return XRS_OK;
+        case XRS_OP_CONVOLVE:
+        case XRS_OP_FOCAL_STAT:
+            XRS_REQUIRE(in_dtype == XRS_F32, "convolve and focal statistics take float32 cells");
+            XRS_REQUIRE(p && aux, "kernel parameters missing");
+            sh->radius = (int)p[0] / 2;
+            return XRS_OK;
+    }
+    set_error("unknown op %d", op);
+    return XRS_EINVAL;
+}
+
 static int run_op(int op, int in_dtype, const void *din, void *dout, int64_t pitch, int64_t opitch, int64_t h,
                   int64_t W, const double *p, const double *aux, int naux, cudaStream_t s) {
-    if (in_dtype != XRS_F32)  // raw int16 / uint16 / int32 / float64 cells: direct-ingest kernels
+    if (in_dtype != XRS_F32 && op != XRS_OP_FOCAL_MEAN)  // raw int16 / uint16 / int32 / float64 cells
         return xrs_surface_typed(op, din, in_dtype, pitch, (float *)dout, opitch, h, W, p, s);
     const float *fi = (const float *)din;
     float *fo = (float *)dout;
@@ -70,10 +111,9 @@ static int run_op(int op, int in_dtype, const void *din, void *dout, int64_t pit
         case XRS_OP_ASPECT: return xrs_aspect_f32(fi, pitch, fo, opitch, h, W, s);
         case XRS_OP_CURVATURE: return xrs_curvature_f32(fi, pitch, fo, opitch, h, W, p[0], s);
         case XRS_OP_HILLSHADE: return xrs_hillshade_f32(fi, pitch, fo, opitch, h, W, p[0], p[1], s);
-        case XRS_OP_FOCAL_MEAN: return xrs_focal_mean_f32(fi, pitch, fo, opitch, h, W, aux, naux, s);
-        case XRS_OP_FOCAL_MEAN_F64:
-            return xrs_focal_mean_f64((const double *)din, pitch, (double *)dout, opitch, h, W, aux, naux, s);
-        case XRS_OP_FOCAL_MEAN_F32_F64:
+        case XRS_OP_FOCAL_MEAN:
+            if (in_dtype == XRS_F64)
+                return xrs_focal_mean_f64((const double *)din, pitch, (double *)dout, opitch, h, W, aux, naux, s);
             return xrs_focal_mean_f32_f64(fi, pitch, (double *)dout, opitch, h, W, aux, naux, s);
         case XRS_OP_CONVOLVE: return xrs_convolve2d_f32(fi, pitch, fo, opitch, h, W, aux, (int)p[0], (int)p[1], s);
         case XRS_OP_FOCAL_STAT:
@@ -87,30 +127,10 @@ static int run_op(int op, int in_dtype, const void *din, void *dout, int64_t pit
 
 using namespace xrs;
 
-// Output rows [y_begin, y_end) of the H x W raster on `device`.
-static int host_pipeline(int op, int in_dtype, const void *in, void *out, int64_t H, int64_t W, const double *p,
-                         const double *aux, int naux, int device, int64_t y_begin = 0, int64_t y_end = -1) {
-    if (y_end < 0) y_end = H;
-    if (H <= 0 || W <= 0 || y_end <= y_begin) return XRS_OK;
-    XRS_REQUIRE(in && out, "NULL host pointer");
-    XRS_REQUIRE(device >= 0 && device < 16, "device index out of range");
-    XRS_REQUIRE(op >= XRS_OP_SLOPE && op <= XRS_OP_FOCAL_MEAN_F32_F64, "unknown op");
-    int esz = (op == XRS_OP_FOCAL_MEAN_F64) ? 8 : 4;                                             // input
-    if (in_dtype != XRS_F32) {
-        XRS_REQUIRE(op <= XRS_OP_HILLSHADE, "typed input is served for slope, aspect, curvature, hillshade");
-        XRS_REQUIRE(W % 4 == 0, "typed host input needs W % 4 == 0");
-        esz = (in_dtype == XRS_F64) ? 8 : (in_dtype == XRS_I32 ? 4 : 2);
-    }
-    const int osz = (op == XRS_OP_FOCAL_MEAN_F64 || op == XRS_OP_FOCAL_MEAN_F32_F64) ? 8 : 4;  // output
-    int radius = 1;
-    if (op == XRS_OP_CONVOLVE || op == XRS_OP_FOCAL_STAT) {
-        XRS_REQUIRE(p && aux, "kernel parameters missing");
-        radius = (int)p[0] / 2;
-    }
-    if ((op == XRS_OP_SLOPE || op == XRS_OP_CURVATURE || op == XRS_OP_HILLSHADE) && !p) {
-        set_error("scalar parameters missing");
-        return XRS_EINVAL;
-    }
+// Output rows [y_begin, y_end) of the H x W raster on `device`; the request was checked by host_op_shape.
+static int host_pipeline(int op, int in_dtype, const OpShape &sh, const void *in, void *out, int64_t H, int64_t W,
+                         const double *p, const double *aux, int naux, int device, int64_t y_begin, int64_t y_end) {
+    const int radius = sh.radius;
     int prev = 0;
     XRS_CUDA(cudaGetDevice(&prev));
     XRS_CUDA(cudaSetDevice(device));
@@ -120,7 +140,7 @@ static int host_pipeline(int op, int in_dtype, const void *in, void *out, int64_
     if (rc) { cudaSetDevice(prev); return rc; }
 
     // device row pitch: multiple of 16 bytes so the TMA kernels apply whenever W % 4 == 0
-    const int64_t row_bytes = W * esz, orow_bytes = W * osz;
+    const int64_t row_bytes = W * sh.in_size, orow_bytes = W * sh.out_size;
     const int64_t pitch = (row_bytes + 15) / 16 * 16, opitch = (orow_bytes + 15) / 16 * 16;
     const int64_t span = y_end - y_begin;
     int64_t rows = (32LL << 20) / pitch;
@@ -166,29 +186,25 @@ static int host_pipeline(int op, int in_dtype, const void *in, void *out, int64_
     return rc;
 }
 
-extern "C" int xrs_host_stencil(int op, const void *in, void *out, int64_t H, int64_t W, const double *p,
-                                const double *aux, int naux, int device) {
-    return host_pipeline(op, XRS_F32, in, out, H, W, p, aux, naux, device);
-}
-
 // Row stripes over several devices, one host thread and one PCIe link per device.  Errors: the
 // first failing stripe's status and message are returned (the message is copied out of the worker
 // thread, whose thread-local error string the caller cannot see).
-static int host_multi(int op, int in_dtype, const void *in, void *out, int64_t H, int64_t W, const double *p,
-                      const double *aux, int naux, const int *devices, int n_devices) {
+extern "C" int xrs_host_stencil(int op, const void *in, int in_dtype, void *out, int64_t H, int64_t W,
+                                const double *p, const double *aux, int naux, const int *devices, int n_devices) {
     XRS_REQUIRE(devices != nullptr && n_devices >= 1 && n_devices <= 16, "1 .. 16 devices expected");
-    if (H <= 0 || W <= 0) return XRS_OK;
-    int radius = 1;
-    if (op == XRS_OP_CONVOLVE || op == XRS_OP_FOCAL_STAT) {
-        XRS_REQUIRE(p != nullptr, "kernel parameters missing");
-        radius = (int)p[0] / 2;
+    for (int i = 0; i < n_devices; ++i) {
+        XRS_REQUIRE(devices[i] >= 0 && devices[i] < 16, "device index out of range");
+        for (int j = 0; j < i; ++j) XRS_REQUIRE(devices[i] != devices[j], "device listed twice");
     }
+    OpShape sh;
+    const int bad = host_op_shape(op, in_dtype, p, aux, W, &sh);
+    if (bad) return bad;
+    if (H <= 0 || W <= 0) return XRS_OK;
+    XRS_REQUIRE(in && out, "NULL host pointer");
     // stripes shorter than a few halos are not worth a device
     int n = n_devices;
-    while (n > 1 && H / n < 8 * radius + 8) --n;
-    if (n == 1) return host_pipeline(op, in_dtype, in, out, H, W, p, aux, naux, devices[0]);
-    for (int i = 0; i < n; ++i)
-        for (int j = 0; j < i; ++j) XRS_REQUIRE(devices[i] != devices[j], "device listed twice");
+    while (n > 1 && H / n < 8 * sh.radius + 8) --n;
+    if (n == 1) return host_pipeline(op, in_dtype, sh, in, out, H, W, p, aux, naux, devices[0], 0, H);
     std::vector<int> rc(n, XRS_OK);
     std::vector<std::string> msg(n);
     std::vector<std::thread> th;
@@ -199,7 +215,7 @@ static int host_multi(int op, int in_dtype, const void *in, void *out, int64_t H
         const int64_t y0 = y, y1 = y + h;
         y = y1;
         th.emplace_back([&, i, y0, y1] {
-            rc[i] = host_pipeline(op, in_dtype, in, out, H, W, p, aux, naux, devices[i], y0, y1);
+            rc[i] = host_pipeline(op, in_dtype, sh, in, out, H, W, p, aux, naux, devices[i], y0, y1);
             if (rc[i] != XRS_OK) msg[i] = xrs_last_error_string();
         });
     }
@@ -210,27 +226,6 @@ static int host_multi(int op, int in_dtype, const void *in, void *out, int64_t H
             return rc[i];
         }
     return XRS_OK;
-}
-
-extern "C" int xrs_host_stencil_multi(int op, const void *in, void *out, int64_t H, int64_t W, const double *p,
-                                      const double *aux, int naux, const int *devices, int n_devices) {
-    return host_multi(op, XRS_F32, in, out, H, W, p, aux, naux, devices, n_devices);
-}
-
-extern "C" int xrs_host_surface_typed_multi(int op, const void *in, int in_dtype, float *out, int64_t H, int64_t W,
-                                            const double *p, const int *devices, int n_devices) {
-    XRS_REQUIRE(in_dtype == XRS_F64 || in_dtype == XRS_I32 || in_dtype == XRS_I16 || in_dtype == XRS_U16,
-                "in_dtype must be int16, uint16, int32 or float64");
-    return host_multi(op, in_dtype, in, out, H, W, p, nullptr, 0, devices, n_devices);
-}
-
-// slope / aspect / curvature / hillshade on a HOST raster of int16 / uint16 / int32 / float64 cells:
-// the raw cells travel over PCIe (half the bytes for 16-bit DEMs) and are converted on the device.
-extern "C" int xrs_host_surface_typed(int op, const void *in, int in_dtype, float *out, int64_t H, int64_t W,
-                                      const double *p, int device) {
-    XRS_REQUIRE(in_dtype == XRS_F64 || in_dtype == XRS_I32 || in_dtype == XRS_I16 || in_dtype == XRS_U16,
-                "in_dtype must be int16, uint16, int32 or float64");
-    return host_pipeline(op, in_dtype, in, out, H, W, p, nullptr, 0, device);
 }
 
 // release the per-device staging buffers (tests / interpreter shutdown)

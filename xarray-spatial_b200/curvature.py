@@ -1,13 +1,12 @@
 """xrspatial.curvature on the CUDA backend (reference: curvature.py:111-247)."""
 from ._xr import DataArray
 from .dataset_support import supports_dataset
-from .utils import (ArrayTypeFunctionMapping, get_dataarray_resolution, run_surface_device,
-                    run_surface_host)
+from .utils import ArrayTypeFunctionMapping, get_dataarray_resolution, run_stencil_host, run_surface_device
 
 
 def _run_numpy(data, cellsize):
-    """replaces curvature.py:44 `_run_numpy`."""
-    return run_surface_host("curvature", data, (cellsize,))
+    """Host raster -> xrs_host_stencil(XRS_OP_CURVATURE) (replaces curvature.py:44 `_run_numpy`)."""
+    return run_stencil_host("curvature", data, (cellsize,))
 
 
 def _run_cupy(data, cellsize):

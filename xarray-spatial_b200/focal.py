@@ -14,8 +14,8 @@ from . import _lib
 from ._xr import DataArray, concat
 from .convolution import custom_kernel
 from .dataset_support import supports_dataset
-from .utils import (ArrayTypeFunctionMapping, _dbl_array, as_device_tensor, is_device_array,
-                    like_container, run_stencil_device, run_stencil_host)
+from .utils import (ArrayTypeFunctionMapping, _dbl_array, as_device_tensor, device_2d, is_device_array,
+                    like_container, run_stencil_device, run_stencil_host, stream_ptr)
 
 
 class _Reducer(object):
@@ -57,22 +57,17 @@ def _stat_of(func):
 def _mean_numpy(data, excludes):
     """One pass on a host raster, float64 result (replaces focal.py:44 `_mean_numpy` after the
     `astype(float)` of focal.py:257; a float32 raster is widened inside the kernel)."""
-    if data.dtype == np.float32:
-        return run_stencil_host("focal_mean_f32_f64", data, aux=tuple(excludes), out_dtype=np.float64,
-                                in_dtype=np.float32)
-    return run_stencil_host("focal_mean_f64", data, aux=tuple(excludes), out_dtype=np.float64,
-                            in_dtype=np.float64)
+    return run_stencil_host("focal_mean", data, aux=tuple(excludes))
 
 
 def _mean_cupy(data, excludes):
     """One pass on a device raster (replaces focal.py:135 `_mean_cupy`): float32 like the
     reference's GPU path, float64 if the input is float64."""
     import torch
-    t = as_device_tensor(data)
     ex = _dbl_array(tuple(excludes))
-    if t.dtype == torch.float64:
-        return run_stencil_device("xrs_focal_mean_f64", data, aux=ex, naux=len(excludes), dtype=torch.float64)
-    return run_stencil_device("xrs_focal_mean_f32", data, aux=ex, naux=len(excludes))
+    if as_device_tensor(data).dtype == torch.float64:
+        return run_stencil_device("xrs_focal_mean_f64", data, ex, len(excludes), dtype=torch.float64)
+    return run_stencil_device("xrs_focal_mean_f32", data, ex, len(excludes))
 
 
 def _mean(data, excludes):
@@ -95,7 +90,7 @@ def mean(agg, passes=1, excludes=[np.nan], name='mean'):
         else:
             # keep intermediate passes on the device: one upload, `passes` kernels, one download
             import torch
-            cur = torch.from_numpy(np.ascontiguousarray(data, dtype=np.float64)).cuda()
+            cur = device_2d(data, torch.float64)
             for _ in range(passes):
                 cur = _mean_cupy(cur, excludes)
             out = cur.cpu().numpy()
@@ -123,8 +118,8 @@ def _apply_numpy(data, kernel, func):
 def _apply_cupy(data, kernel, func):
     """device raster -> xrs_focal_stat_f32 with the CPU (NaN-skipping) semantics."""
     k = np.ascontiguousarray(kernel, dtype=np.float64)
-    return run_stencil_device("xrs_focal_stat_f32", data, aux=k.ctypes.data_as(ctypes.c_void_p),
-                              extra_ints=(k.shape[0], k.shape[1], _lib.STATS[_stat_of(func)]))
+    return run_stencil_device("xrs_focal_stat_f32", data, k.ctypes.data_as(ctypes.c_void_p), k.shape[0], k.shape[1],
+                              _lib.STATS[_stat_of(func)])
 
 
 def apply(raster, kernel, func=_calc_mean, name='focal_apply'):
@@ -144,8 +139,7 @@ def _focal_stats_cupy(data, kernel, stats_funcs):
     """device raster -> (stats, y, x) stack from ONE pass (xrs_focal_stats_multi_f32); replaces
     focal.py:757 `_focal_stats_cupy`, with the CPU (NaN-skipping, kernel == 1) semantics."""
     import torch
-    from .utils import device_f32_2d, stream_ptr
-    t = device_f32_2d(data)
+    t = device_2d(data, torch.float32)
     H, W = t.shape
     k = np.ascontiguousarray(kernel, dtype=np.float64)
     ids = (ctypes.c_int * len(stats_funcs))(*[_lib.STATS[s] for s in stats_funcs])
@@ -190,8 +184,7 @@ def _hotspots_device(data, kernel):
     mean / std, classify (replaces focal.py:918-937 `_hotspots_numpy` / :1025 `_hotspots_cupy`)."""
     import torch
     from .convolution import _convolve_2d_cupy
-    from .utils import device_f32_2d, stream_ptr
-    t = device_f32_2d(data)
+    t = device_2d(data, torch.float32)
     k = np.asarray(kernel, dtype=np.float64)
     mean_array = as_device_tensor(_convolve_2d_cupy(t, k / k.sum()))
     part = torch.empty(3, dtype=torch.float64, device=t.device)
@@ -232,9 +225,7 @@ def hotspots(raster, kernel):
     if kind is not None and kind not in "iuf":
         raise ValueError("data type must be integer or float")
     if isinstance(raster.data, np.ndarray):
-        import torch
-        out = _hotspots_device(torch.from_numpy(np.ascontiguousarray(raster.data, dtype=np.float32)).cuda(), kernel)
-        out = out.cpu().numpy()
+        out = _hotspots_device(raster.data, kernel).cpu().numpy()
     elif is_device_array(raster.data):
         out = like_container(_hotspots_device(raster.data, kernel), raster.data)
     else:

@@ -3,14 +3,14 @@ import numpy as np
 
 from ._xr import DataArray
 from .dataset_support import supports_dataset
-from .utils import is_dask_array, is_device_array, run_surface_device, run_surface_host
+from .utils import is_dask_array, is_device_array, run_stencil_host, run_surface_device
 
 
 def _run_numpy(data, azimuth=225, angle_altitude=25):
     """replaces hillshade.py:20 `_run_numpy`.  Returns float32 (the dtype the reference
     documents and its GPU path produces; its NumPy path yields float64 only through NumPy-2
     scalar promotion, SURVEY.md 8a row a5)."""
-    return run_surface_host("hillshade", data, (azimuth, angle_altitude))
+    return run_stencil_host("hillshade", data, (azimuth, angle_altitude))
 
 
 def _run_cupy(d_data, azimuth, angle_altitude):

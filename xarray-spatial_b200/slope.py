@@ -2,12 +2,12 @@
 from ._xr import DataArray
 from .dataset_support import supports_dataset
 from .utils import (Z_UNITS, ArrayTypeFunctionMapping, extract_latlon, get_dataarray_resolution,
-                    run_geodesic, run_surface_device, run_surface_host)
+                    run_geodesic, run_stencil_host, run_surface_device)
 
 
 def _run_numpy(data, cellsize_x, cellsize_y):
     """Host raster -> xrs_host_stencil(XRS_OP_SLOPE) (replaces slope.py:79 `_run_numpy`)."""
-    return run_surface_host("slope", data, (cellsize_x, cellsize_y))
+    return run_stencil_host("slope", data, (cellsize_x, cellsize_y))
 
 
 def _run_cupy(data, cellsize_x, cellsize_y):

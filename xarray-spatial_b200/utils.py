@@ -89,10 +89,6 @@ def host_devices():
     return devs
 
 
-def _dev_array(devs):
-    return (ctypes.c_int * len(devs))(*devs), len(devs)
-
-
 def not_implemented_func(agg, *args, messages='Not yet implemented.'):
     raise NotImplementedError(messages)
 
@@ -178,49 +174,43 @@ def _dbl_array(vals):
     return arr
 
 
-def device_f32_2d(data):
-    """(tensor, template): 2-D float32 CUDA tensor with unit inner stride (cast/copy only if
-    needed, like the reference's `data.astype(cupy.float32)`, slope.py:150)."""
+def device_2d(data, dtype=None):
+    """2-D CUDA tensor with unit inner stride, cast to `dtype` when given (like the reference's
+    `data.astype(cupy.float32)`, slope.py:150).  A numpy raster is cast on the host and uploaded; a
+    device array is viewed, and cast or copied only if needed."""
+    if isinstance(data, np.ndarray):
+        if data.ndim != 2:
+            raise ValueError("expected a 2-D raster, got %d-D" % data.ndim)
+        np_dtype = None if dtype is None else torch.empty(0, dtype=dtype).numpy().dtype
+        return torch.from_numpy(np.ascontiguousarray(data, dtype=np_dtype)).cuda()
     t = as_device_tensor(data)
     if t.dim() != 2:
         raise ValueError("expected a 2-D raster, got %d-D" % t.dim())
-    if t.dtype != torch.float32:
-        t = t.to(torch.float32)
+    if dtype is not None and t.dtype != dtype:
+        t = t.to(dtype)
     if t.numel() and t.stride(1) != 1:
         t = t.contiguous()
     return t
 
 
-def run_stencil_device(fn_name, data, *scalars, aux=None, naux=None, extra_ints=(), dtype=None):
-    """Call a `(in, pitch, out, pitch, H, W, ...)` device entry point on torch's current stream."""
-    if dtype is None:
-        t = device_f32_2d(data)
-    else:
-        t = as_device_tensor(data)
-        if t.dtype != dtype:
-            t = t.to(dtype)
-        if t.numel() and t.stride(1) != 1:
-            t = t.contiguous()
+def run_stencil_device(fn_name, data, *args, dtype=None):
+    """Call the device entry point `fn_name(in, in_pitch, out, out_pitch, H, W, *args, stream)` on
+    torch's current stream, `args` being its own arguments in header order.  The raster is cast to
+    `dtype` (default float32) and the result has the same dtype."""
+    t = device_2d(data, dtype or torch.float32)
     H, W = t.shape
     out = torch.empty((H, W), dtype=t.dtype, device=t.device)
     if H == 0 or W == 0:
         return like_container(out, data)
     esz = t.element_size()
-    args = [ctypes.c_void_p(t.data_ptr()), t.stride(0) * esz, ctypes.c_void_p(out.data_ptr()),
-            out.stride(0) * esz, H, W]
-    args += [float(s) for s in scalars]
-    if aux is not None:
-        args += [aux]
-        if naux is not None:
-            args += [int(naux)]
-    args += [int(i) for i in extra_ints]
     with torch.cuda.device(t.device):
-        args.append(stream_ptr(t))
-        _lib.call(fn_name, *args)
+        _lib.call(fn_name, ctypes.c_void_p(t.data_ptr()), t.stride(0) * esz, ctypes.c_void_p(out.data_ptr()),
+                  out.stride(0) * esz, H, W, *args, stream_ptr(t))
     return like_container(out, data)
 
 
-_INGEST_NP = {"int16": 4, "uint16": 5, "int32": 2, "float64": 1}
+_SURFACE_OPS = ("slope", "aspect", "curvature", "hillshade")
+_SURFACE_CELLS = ("int16", "uint16", "int32", "float64")   # what the direct-ingest kernels read
 
 
 def run_surface_device(op, fn_name, data, *scalars):
@@ -228,53 +218,46 @@ def run_surface_device(op, fn_name, data, *scalars):
     rasters go through the direct-ingest kernels (xrs_surface_typed: no separate cast pass); other
     dtypes are cast to float32 first, like the reference does (slope.py:150)."""
     t = as_device_tensor(data)
-    code = _INGEST_NP.get(str(t.dtype).replace("torch.", ""))
-    if code is not None and t.dim() == 2 and t.numel() and t.stride(1) == 1:
+    cells = str(t.dtype).replace("torch.", "")
+    if cells in _SURFACE_CELLS and t.dim() == 2 and t.numel() and t.stride(1) == 1:
         H, W = t.shape
         out = torch.empty((H, W), dtype=torch.float32, device=t.device)
         try:
             with torch.cuda.device(t.device):
-                _lib.call("xrs_surface_typed", _lib.OPS[op], ctypes.c_void_p(t.data_ptr()), code,
+                _lib.call("xrs_surface_typed", _lib.OPS[op], ctypes.c_void_p(t.data_ptr()), _lib.DTYPES[cells],
                           t.stride(0) * t.element_size(), ctypes.c_void_p(out.data_ptr()), out.stride(0) * 4, H, W,
                           _dbl_array(scalars), stream_ptr(t))
             return like_container(out, data)
         except NotImplementedError:
             pass  # layout the ingest kernels do not take (odd width, misaligned rows): cast instead
-    return run_stencil_device(fn_name, data, *scalars)
+    return run_stencil_device(fn_name, data, *[float(s) for s in scalars])
 
 
-def run_surface_host(op, data, p=()):
-    """Same for numpy rasters: raw 16-bit / int32 / float64 cells cross PCIe and are converted on the
-    device when the layout allows it, else the raster is cast on the host (slope.py:58)."""
-    from . import _hostmem
-    code = _INGEST_NP.get(data.dtype.name)
-    if code is not None and data.ndim == 2 and data.size and data.shape[1] % 4 == 0:
-        d = np.ascontiguousarray(data)
-        H, W = d.shape
-        out = _hostmem.empty((H, W), np.float32)
-        try:
-            devs, nd = _dev_array(host_devices())
-            _lib.call("xrs_host_surface_typed_multi", _lib.OPS[op], ctypes.c_void_p(d.ctypes.data), code,
-                      ctypes.c_void_p(out.ctypes.data), H, W, _dbl_array(p), devs, nd)
-            return out
-        except NotImplementedError:
-            pass
-    return run_stencil_host(op, data, p)
-
-
-def run_stencil_host(op, data, p=(), aux=(), out_dtype=np.float32, in_dtype=np.float32):
-    """Call xrs_host_stencil on a numpy raster; the result is a numpy array in pinned memory."""
+def run_stencil_host(op, data, p=(), aux=()):
+    """xrs_host_stencil on a numpy raster over host_devices(); the result is a numpy array in pinned
+    memory.  The cells that cross PCIe follow the C entry point's table:
+      * slope / aspect / curvature / hillshade: int16, uint16, int32 and float64 rasters as they are
+        when W % 4 == 0 (converted on the device; half the bytes for 16-bit DEMs), anything else cast
+        to float32 (slope.py:58); float32 result;
+      * focal mean: float32 as it is, anything else cast to float64; float64 result (focal.py:257);
+      * convolve / focal statistics: cast to float32; float32 result."""
     from . import _hostmem
     if data.ndim != 2:
         raise ValueError("expected a 2-D raster, got %d-D" % data.ndim)
-    d = np.ascontiguousarray(data, dtype=in_dtype)
-    H, W = d.shape
+    H, W = data.shape
+    cells, out_dtype = "float32", np.float32
+    if op == "focal_mean":
+        cells, out_dtype = ("float32" if data.dtype.name == "float32" else "float64"), np.float64
+    elif op in _SURFACE_OPS and data.dtype.name in _SURFACE_CELLS and W % 4 == 0:
+        cells = data.dtype.name
     if H == 0 or W == 0:
         return np.empty((H, W), out_dtype)
+    d = np.ascontiguousarray(data, dtype=cells)
     out = _hostmem.empty((H, W), out_dtype)
-    devs, nd = _dev_array(host_devices())
-    _lib.call("xrs_host_stencil_multi", _lib.OPS[op], ctypes.c_void_p(d.ctypes.data),
-              ctypes.c_void_p(out.ctypes.data), H, W, _dbl_array(p), _dbl_array(aux), len(aux), devs, nd)
+    devs = host_devices()
+    _lib.call("xrs_host_stencil", _lib.OPS[op], ctypes.c_void_p(d.ctypes.data), _lib.DTYPES[cells],
+              ctypes.c_void_p(out.ctypes.data), H, W, _dbl_array(p), _dbl_array(aux), len(aux),
+              (ctypes.c_int * len(devs))(*devs), len(devs))
     return out
 
 
@@ -343,17 +326,9 @@ def extract_latlon(agg):
 
 def run_geodesic(data, lat, lon, is_2d, z_factor, want_aspect):
     """xrs_geodesic on a device or host raster; result in the container type of `data`."""
-    host_in = isinstance(data, np.ndarray)
-    if host_in:
-        t = torch.from_numpy(np.ascontiguousarray(data)).cuda()
-    else:
-        t = as_device_tensor(data)
-    if t.dim() != 2:
-        raise ValueError("expected a 2-D raster, got %d-D" % t.dim())
+    t = device_2d(data)
     if t.dtype not in (torch.float32, torch.float64):
         t = t.to(torch.float64)           # the reference computes on data.astype(float64), slope.py:169
-    if t.numel() and t.stride(1) != 1:
-        t = t.contiguous()
     H, W = t.shape
     out = torch.empty((H, W), dtype=torch.float32, device=t.device)
     if H and W:
@@ -364,6 +339,6 @@ def run_geodesic(data, lat, lon, is_2d, z_factor, want_aspect):
                       t.stride(0) * t.element_size(), ctypes.c_void_p(lat_t.data_ptr()),
                       ctypes.c_void_p(lon_t.data_ptr()), 1 if is_2d else 0, ctypes.c_void_p(out.data_ptr()),
                       out.stride(0) * 4, H, W, float(z_factor), 1 if want_aspect else 0, stream_ptr(t))
-    if host_in:
+    if isinstance(data, np.ndarray):
         return out.cpu().numpy()
     return like_container(out, data)
