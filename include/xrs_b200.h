@@ -12,7 +12,8 @@
  * Conventions
  *  - plain C types only; rasters are row-major (H rows = y, W cols = x); pitches in BYTES.
  *  - `*_f32` device entry points take DEVICE pointers and a cudaStream_t (as void*), only
- *    enqueue work on that stream and never synchronise or allocate user-visible memory.
+ *    enqueue work on that stream and never synchronise or allocate user-visible memory (the one
+ *    exception, convolve / focal statistics over wide windows, is described at those functions).
  *  - `xrs_host_*` entry points take HOST pointers (pinned or pageable), run the same kernels
  *    through an internal pipelined H2D / compute / D2H stripe engine, and return when the
  *    result is in `out`.  They are what a numpy-backed DataArray call uses.
@@ -116,7 +117,12 @@ int xrs_focal_mean_f32_f64(const float *in, int64_t in_pitch, double *out, int64
                            int64_t H, int64_t W, const double *excludes, int n_ex,
                            xrs_stream_t s);
 /* convolution._convolve_2d_cupy (convolution.py:368-374) / `_convolve_2d_numpy` (:285-313):
- * correlation with a host float64 kernel (kh, kw odd, <= 63); NaN ring of (kh/2, kw/2). */
+ * correlation with a host float64 kernel (kh, kw odd, 1 .. 2047); NaN ring of (kh/2, kw/2).  Windows of
+ * more than 49 x 49 taps or more than 63 cells on a side run on the wide-window kernel, which copies the
+ * weights into a buffer allocated and freed on `s` (reentrant across streams).  That copy is from pageable
+ * host memory: a table too large for the driver's staging buffers (a 2047 x 2047 window's 33.5 MB of
+ * weights) may hold the call until earlier work on `s` is done, and wide windows cannot be captured into a
+ * CUDA graph. */
 int xrs_convolve2d_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch,
                        int64_t H, int64_t W, const double *kernel, int kh, int kw,
                        xrs_stream_t s);
@@ -124,7 +130,9 @@ int xrs_convolve2d_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
  * (focal.py:305-326) + reducers (:268-302): cells where kernel == 1 participate, NaN and
  * out-of-raster cells are skipped.  `stat` is an xrs_focal_stat.  XRS_STAT_MEAN over a kernel of all
  * ones (np.ones((kh, kw)), the reference's FocalApply benchmark; odd kh, kw <= 25) runs on the running-box
- * kernel in NaN-skipping mode, O(1) work per cell; everything else on the tiled kernels. */
+ * kernel in NaN-skipping mode, O(1) work per cell; windows up to 49 x 49 taps and 63 per side on the tiled
+ * kernels; wider ones (odd kh, kw up to 2047) on the wide-window kernel, with the mask in a buffer allocated
+ * and freed on `s`. */
 int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch,
                        int64_t H, int64_t W, const double *kernel, int kh, int kw, int stat,
                        xrs_stream_t s);
@@ -132,7 +140,8 @@ int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
  * plane i of `out` (planes `plane_stride` bytes apart, rows `out_pitch` bytes apart) receives
  * statistic stats[i] (xrs_focal_stat ids, no duplicates, n_stats <= 7).  The tile is loaded
  * once and swept twice for all seven statistics; results are bit-identical to n_stats calls
- * of xrs_focal_stat_f32. */
+ * of xrs_focal_stat_f32.  Windows beyond 49 x 49 taps or 63 per side (odd sides up to 2047) take the
+ * fused wide-window kernel: one sweep for mean / sum / min / max / range, a second only for var / std. */
 int xrs_focal_stats_multi_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch,
                               int64_t plane_stride, int64_t H, int64_t W, const double *kernel,
                               int kh, int kw, const int *stats, int n_stats, xrs_stream_t s);
@@ -255,7 +264,8 @@ int xrs_host_free(void *ptr);
  * kernel, 1 TMA strip kernel, 2 direct-ingest TMA kernel, 3 running-box kernel (uniform convolve_2d, focal.apply
  * mean over an all-ones window), 4 generic tiled convolve, 5 bounds-checked convolve fallback, 6 fused focal
  * statistics, 7 tiled single focal statistic, 8 bounds-checked focal statistic fallback, 9 zonal group-by
- * (xrs_zonal_hash_run / _second_pass), 10 zonal pair count (xrs_zonal_pair_count) -- and with how many CTAs */
+ * (xrs_zonal_hash_run / _second_pass), 10 zonal pair count (xrs_zonal_pair_count), 11 wide-window convolve,
+ * 12 wide-window single focal statistic, 13 wide-window fused focal statistics -- and with how many CTAs */
 int xrs_debug_last_used_tma(void);
 int xrs_debug_last_grid(void);
 /* host-only test hook: the row-segment height the persistent kernels pick for a raster of H rows cut into

@@ -30,6 +30,9 @@ enum LaunchKind : int {
     kFocalDirect = 8,   // bounds-checked single focal statistic
     kZonalHash = 9,     // zonal group-by
     kZonalPair = 10,    // zonal (zone, value) pair count
+    kConvWide = 11,     // convolve over a window beyond the tiled kernels (conv.cu, "wide windows")
+    kFocalWide = 12,    // single focal statistic over such a window
+    kFocalWideFused = 13,  // every requested focal statistic over such a window
 };
 
 struct LaunchInfo {  // for tests / profiling: what the last launch on this thread chose
@@ -51,6 +54,10 @@ LaunchInfo &last_launch_info();
             return XRS_EINVAL;                     \
         }                                          \
     } while (0)
+
+// XRS_EINVAL with a message unless kh and kw are odd and 1 .. 2047: the windows of convolve and the focal
+// statistics (conv.cu)
+int check_window(int kh, int kw);
 
 // cached per-device properties
 int sm_count(int device = -1);

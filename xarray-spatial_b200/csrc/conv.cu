@@ -14,6 +14,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <vector>
+
 #include "common.cuh"
 
 namespace xrs {
@@ -611,12 +613,373 @@ focal_stat_direct_kernel(const float *__restrict__ in, int64_t in_pitch_elems, c
     }
 }
 
+// ----------------------------------------------------------------------------- wide windows
+// Windows beyond the tiled kernels' reach (more than kMaxTaps taps, or a side above 63): the weights and
+// the mask no longer fit the kernel-parameter bank, and the (tile + halo) block no longer fits shared
+// memory.  A CTA owns 4 output rows x kWideConvW (convolve) or kWideStatW (statistics) columns and streams
+// the kh + 3 input rows of its window through a ring of kRing shared-memory rows, filled by bounds-checked
+// cp.async loads (any pitch, offset or width; out-of-raster cells NaN).  Input row J feeds output row r
+// with kernel row J - r, uniform across the CTA, so every output receives its taps in row-major order,
+// like the tiled kernels, and a thread's 4 x 8 (convolve) or 4 x 4 (statistics) outputs share each
+// loaded cell.  The weights (kh rows of kwp doubles) and the mask (per kernel row: the [lo, hi) span of
+// its ones and a bit row) live in a stream-ordered device buffer made for the call.
+constexpr int kWideSide = 2047;
+constexpr int kWideConvW = 2048, kWideStatW = 1024, kRing = 4;
+constexpr int kAllStats = -1;  // focal_wide_kernel: every statistic whose plane is set
+
+struct WideGeom {
+    int64_t H, W, in_pitch, out_pitch;  // pitches in cells
+    int kh, kw;
+    int kwp;                            // kw rounded up to 4: weight row stride, and the chunk loops' bound
+    int nw;                             // mask words per kernel row
+    int rw;                             // cells per ring row (multiple of 4)
+    int tiles_x;
+    int64_t n_tiles;
+};
+
+__device__ __forceinline__ void cp_async4(float *dst, const float *src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() {
+    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// Raster row y, columns xs .. xs + rw - 1, into ring row `slot`; out-of-raster cells are NaN.
+__device__ __forceinline__ void ring_load(float *ring, const float *__restrict__ in, const WideGeom &g, int64_t y,
+                                          int64_t xs, int slot) {
+    float *dst = ring + (size_t)slot * g.rw;
+    const bool row_in = y >= 0 && y < g.H;
+    for (int i = threadIdx.x; i < g.rw; i += blockDim.x) {
+        const int64_t x = xs + i;
+        if (row_in && x >= 0 && x < g.W) cp_async4(dst + i, in + y * g.in_pitch + x);
+        else dst[i] = nan_of<float>();
+    }
+}
+
+// Streams input rows J = 0 .. kh + 2 (raster rows y0 - kh/2 + J) through the ring, kRing - 1 rows ahead of
+// the one `fn(J, row)` consumes.
+template <typename F>
+__device__ __forceinline__ void ring_sweep(float *ring, const float *__restrict__ in, const WideGeom &g, int64_t y0,
+                                           int64_t xs, F &&fn) {
+    const int rows = g.kh + 3;
+    const int64_t ya = y0 - g.kh / 2;
+#pragma unroll
+    for (int j = 0; j < kRing - 1; ++j) {
+        if (j < rows) ring_load(ring, in, g, ya + j, xs, j);
+        cp_async_commit();
+    }
+    for (int j = 0; j < rows; ++j) {
+        cp_async_wait<kRing - 2>();
+        __syncthreads();  // row j has landed everywhere, and every thread is done with row j - 1
+        if (j + kRing - 1 < rows) ring_load(ring, in, g, ya + j + kRing - 1, xs, (j + kRing - 1) % kRing);
+        cp_async_commit();
+        fn(j, ring + (size_t)(j % kRing) * g.rw);
+    }
+    __syncthreads();  // the next sweep refills the ring
+}
+
+// A thread owns output rows y0 .. y0 + 3 and columns base + 0..3 and base + 64 + 0..3: consecutive lanes read
+// consecutive 16-byte pieces of a ring row (conflict-free LDS.128), as in conv2d_kernel.
+__global__ void __launch_bounds__(256)
+conv2d_wide_kernel(const float *__restrict__ in, const double *__restrict__ w, float *__restrict__ out,
+                   const WideGeom g) {
+    extern __shared__ __align__(16) float ring[];
+    const int base = 128 * (threadIdx.x >> 4) + 4 * (threadIdx.x & 15);
+    const int kw4 = g.kw & ~3;
+    for (int64_t t = blockIdx.x; t < g.n_tiles; t += gridDim.x) {
+        const int64_t y0 = t / g.tiles_x * 4, x0 = t % g.tiles_x * kWideConvW;
+        double acc[4][8];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 8; ++c) acc[r][c] = 0.0;
+        ring_sweep(ring, in, g, y0, x0 - g.kw / 2, [&](int j, const float *row) {
+            const float *rowp = row + base;
+            // taps kb .. kb + nt - 1 of the kernel rows j - r, one half of the thread's columns at a time.  Each
+            // cell is widened once per chunk: left alone, the compiler sinks the F2F.F64 into every kernel-row
+            // branch, and F2F.F64 issues at a quarter of the DFMA rate; the empty asm pins the widened value.
+            auto chunk = [&](const int kb, const int nt) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float4 a0 = *reinterpret_cast<const float4 *>(rowp + 64 * h + kb);
+                    const float4 a1 = *reinterpret_cast<const float4 *>(rowp + 64 * h + kb + 4);
+                    double v[8] = {(double)a0.x, (double)a0.y, (double)a0.z, (double)a0.w,
+                                   (double)a1.x, (double)a1.y, (double)a1.z, (double)a1.w};
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) asm("" : "+d"(v[i]));
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) {
+                        const int ky = j - r;
+                        if (ky >= 0 && ky < g.kh) {  // CTA-uniform
+                            const double2 *wr = reinterpret_cast<const double2 *>(w + (int64_t)ky * g.kwp + kb);
+                            const double2 w01 = __ldg(wr), w23 = __ldg(wr + 1);
+                            const double wv[4] = {w01.x, w01.y, w23.x, w23.y};
+#pragma unroll
+                            for (int tt = 0; tt < 4; ++tt)
+                                if (tt < nt)
+#pragma unroll
+                                    for (int c = 0; c < 4; ++c)
+                                        acc[r][4 * h + c] = fma(wv[tt], v[c + tt], acc[r][4 * h + c]);
+                        }
+                    }
+                }
+            };
+            for (int kb = 0; kb < kw4; kb += 4) chunk(kb, 4);
+            if (kw4 < g.kw) chunk(kw4, g.kw - kw4);
+        });
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int64_t yo = y0 + r;
+            if (yo >= g.H) continue;
+            float *orow = out + yo * g.out_pitch;
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+                const int64_t xo = x0 + base + (c & 3) + (c >> 2) * 64;
+                if (xo < g.W) orow[xo] = (float)acc[r][c];
+            }
+        }
+    }
+}
+
+// The statistics of focal_stat_kernel / focal_stats_multi_kernel, operation for operation, over a thread's
+// 4 x 4 outputs (columns base .. base + 3).  Sweep A: float64 sum, count, float32 sum, min and max; sweep B,
+// only for var / std: the squared deviations about the float64 mean.  STAT is one xrs_focal_stat (one output
+// plane), or kAllStats for every plane that is set.  Each sweep visits, per input row, only the 4-tap chunks inside
+// the union of the spans of ones of the (up to four) kernel rows it feeds.
+template <int STAT>
+__global__ void __launch_bounds__(256)
+focal_wide_kernel(const float *__restrict__ in, const int2 *__restrict__ span, const uint32_t *__restrict__ bits,
+                  const StatPlanes planes, const WideGeom g) {
+    extern __shared__ __align__(16) float ring[];
+    auto want = [&](int s) { return STAT == kAllStats ? planes.p[s] != nullptr : STAT == s; };
+    // what sweep A accumulates: everything for the fused kernel, only what its statistic needs otherwise
+    constexpr bool kSums = STAT == kAllStats || STAT == XRS_STAT_MEAN || STAT == XRS_STAT_SUM ||
+                           STAT == XRS_STAT_VAR || STAT == XRS_STAT_STD;
+    constexpr bool kMinMax = STAT == kAllStats || STAT == XRS_STAT_MIN || STAT == XRS_STAT_MAX ||
+                             STAT == XRS_STAT_RANGE;
+    const int base = 4 * threadIdx.x;
+    for (int64_t t = blockIdx.x; t < g.n_tiles; t += gridDim.x) {
+        const int64_t y0 = t / g.tiles_x * 4, x0 = t % g.tiles_x * kWideStatW, xs = x0 - g.kw / 2;
+        auto sweep = [&](auto &&f) {
+            ring_sweep(ring, in, g, y0, xs, [&](int j, const float *row) {
+                const float *rowp = row + base;
+                int lo = g.kwp, hi = 0;
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    const int ky = j - r;
+                    if (ky >= 0 && ky < g.kh) {
+                        const int2 sp = __ldg(span + ky);
+                        lo = min(lo, sp.x);
+                        hi = max(hi, sp.y);
+                    }
+                }
+                for (int kb = lo; kb < hi; kb += 4) {
+                    const float4 q0 = *reinterpret_cast<const float4 *>(rowp + kb);
+                    const float4 q1 = *reinterpret_cast<const float4 *>(rowp + kb + 4);
+                    const float v[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
+                    FocalCell cell[8];
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        cell[i].v = v[i];
+                        cell[i].ok = (v[i] == v[i]);
+                        cell[i].vz = cell[i].ok ? v[i] : 0.f;
+                        cell[i].d = (double)v[i];
+                        cell[i].dz = (double)cell[i].vz;
+                        cell[i].one = cell[i].ok ? 1 : 0;
+                    }
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) {
+                        const int ky = j - r;
+                        if (ky < 0 || ky >= g.kh) continue;
+                        const uint32_t nib = (__ldg(bits + (int64_t)ky * g.nw + (kb >> 5)) >> (kb & 31)) & 15u;
+                        if (nib == 15u) {  // CTA-uniform
+#pragma unroll
+                            for (int tt = 0; tt < 4; ++tt)
+#pragma unroll
+                                for (int c = 0; c < 4; ++c) f(r, c, cell[c + tt]);
+                        } else if (nib) {
+#pragma unroll
+                            for (int tt = 0; tt < 4; ++tt)
+                                if (nib >> tt & 1u)
+#pragma unroll
+                                    for (int c = 0; c < 4; ++c) f(r, c, cell[c + tt]);
+                        }
+                    }
+                }
+            });
+        };
+        auto store = [&](int s, const float (&res)[4][4]) {
+            float *plane = planes.p[s];
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+                if (y0 + r < g.H)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c)
+                        if (x0 + base + c < g.W) plane[(y0 + r) * g.out_pitch + x0 + base + c] = res[r][c];
+        };
+        float res[4][4];
+        double mean[4][4];
+        int cnt[4][4];
+        float fsum[4][4], mn[4][4], mx[4][4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                mean[r][c] = 0.0, cnt[r][c] = 0, fsum[r][c] = 0.f, mn[r][c] = mx[r][c] = nan_of<float>();
+        sweep([&](int r, int c, const FocalCell &q) {
+            if (kSums) {
+                mean[r][c] += q.dz;
+                cnt[r][c] += q.one;
+                fsum[r][c] += q.vz;
+            }
+            if (kMinMax) {
+                nan_min_step(mn[r][c], q.v);
+                nan_max_step(mx[r][c], q.v);
+            }
+        });
+        if (want(XRS_STAT_SUM)) store(XRS_STAT_SUM, fsum);
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                mean[r][c] = mean[r][c] / (double)cnt[r][c];
+                res[r][c] = (float)mean[r][c];
+            }
+        if (want(XRS_STAT_MEAN)) store(XRS_STAT_MEAN, res);
+        if (want(XRS_STAT_MIN)) store(XRS_STAT_MIN, mn);
+        if (want(XRS_STAT_MAX)) store(XRS_STAT_MAX, mx);
+        if (want(XRS_STAT_RANGE)) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) res[r][c] = mx[r][c] - mn[r][c];
+            store(XRS_STAT_RANGE, res);
+        }
+        if (want(XRS_STAT_VAR) || want(XRS_STAT_STD)) {
+            double ssd[4][4];
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) ssd[r][c] = 0.0;
+            sweep([&](int r, int c, const FocalCell &q) {
+                const double d = q.d - mean[r][c];
+                ssd[r][c] += q.ok ? d * d : 0.0;
+            });
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    ssd[r][c] = ssd[r][c] / (double)cnt[r][c];
+                    res[r][c] = (float)ssd[r][c];
+                }
+            if (want(XRS_STAT_VAR)) store(XRS_STAT_VAR, res);
+            if (want(XRS_STAT_STD)) {
+#pragma unroll
+                for (int r = 0; r < 4; ++r)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) res[r][c] = (float)sqrt(ssd[r][c]);
+                store(XRS_STAT_STD, res);
+            }
+        }
+    }
+}
+
+int check_window(int kh, int kw) {
+    XRS_REQUIRE(kh >= 1 && kw >= 1 && (kh & 1) && (kw & 1), "kernel dimensions must be odd");
+    XRS_REQUIRE(kh <= kWideSide && kw <= kWideSide, "kernel too large (max 2047 cells per side)");
+    return XRS_OK;
+}
+
+static bool is_wide(int kh, int kw) { return kh * kw > kMaxTaps || kh > 63 || kw > 63; }
+
+static WideGeom wide_geom(int64_t in_pitch, int64_t out_pitch, int64_t H, int64_t W, int kh, int kw, int tile_w) {
+    WideGeom g;
+    g.H = H; g.W = W; g.in_pitch = in_pitch / 4; g.out_pitch = out_pitch / 4;
+    g.kh = kh; g.kw = kw;
+    g.kwp = (kw + 3) & ~3;
+    g.nw = (g.kwp + 31) / 32;
+    g.rw = tile_w + g.kwp + 8;  // the 8-cell chunk loads of the last tap chunk reach tile_w + kwp + 3
+    g.tiles_x = (int)((W + tile_w - 1) / tile_w);
+    g.n_tiles = (H + 3) / 4 * g.tiles_x;
+    return g;
+}
+
+// Copies the host table into a buffer ordered on stream s, runs launch_fn(device pointer) and frees the
+// buffer after it on the same stream: concurrent calls on distinct streams each use their own copy.
+template <typename L>
+static int with_device_table(const std::vector<char> &table, cudaStream_t s, L &&launch_fn) {
+    void *d = nullptr;
+    XRS_CUDA(cudaMallocAsync(&d, table.size(), s));
+    const cudaError_t e = cudaMemcpyAsync(d, table.data(), table.size(), cudaMemcpyHostToDevice, s);
+    int rc = e == cudaSuccess ? launch_fn(d) : cuda_fail(e, "cudaMemcpyAsync");
+    const cudaError_t ef = cudaFreeAsync(d, s);
+    if (rc == XRS_OK && ef != cudaSuccess) rc = cuda_fail(ef, "cudaFreeAsync");
+    return rc;
+}
+
+template <typename... P, typename... A>
+static int launch_wide(void (*kern)(P...), const WideGeom &g, cudaStream_t s, LaunchKind kind, const A &...args) {
+    const size_t smem = (size_t)kRing * g.rw * sizeof(float);
+    int64_t resident;
+    if (const int rc = resident_ctas(kern, 256, smem, INT_MAX, &resident)) return rc;
+    return launch(kern, resident < g.n_tiles ? resident : g.n_tiles, 256, smem, s, kind, args...);
+}
+
+static int conv2d_wide(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
+                       const double *kernel, int kh, int kw, cudaStream_t s) {
+    const WideGeom g = wide_geom(in_pitch, out_pitch, H, W, kh, kw, kWideConvW);
+    std::vector<char> table((size_t)kh * g.kwp * sizeof(double), 0);  // kh rows of kwp weights, zero padded
+    double *w = reinterpret_cast<double *>(table.data());
+    for (int ky = 0; ky < kh; ++ky) memcpy(w + (size_t)ky * g.kwp, kernel + (size_t)ky * kw, kw * sizeof(double));
+    return with_device_table(table, s, [&](void *d) {
+        return launch_wide(conv2d_wide_kernel, g, s, kConvWide, in, (const double *)d, out, g);
+    });
+}
+
+// stat: one xrs_focal_stat into planes.p[stat], or kAllStats
+static int focal_wide(const float *in, int64_t in_pitch, const StatPlanes &planes, int64_t out_pitch, int64_t H,
+                      int64_t W, const double *kernel, int kh, int kw, int stat, cudaStream_t s) {
+    const WideGeom g = wide_geom(in_pitch, out_pitch, H, W, kh, kw, kWideStatW);
+    // kh spans [lo, hi) (4-tap chunks holding the row's ones; lo = kwp, hi = 0 for a row without any), then
+    // kh rows of nw mask words
+    const size_t span_bytes = (size_t)kh * sizeof(int2);
+    std::vector<char> table(span_bytes + (size_t)kh * g.nw * sizeof(uint32_t), 0);
+    int2 *span = reinterpret_cast<int2 *>(table.data());
+    uint32_t *bits = reinterpret_cast<uint32_t *>(table.data() + span_bytes);
+    for (int ky = 0; ky < kh; ++ky) {
+        int first = -1, last = -1;
+        for (int kx = 0; kx < kw; ++kx)
+            if (kernel[(size_t)ky * kw + kx] == 1.0) {  // focal.py:323
+                bits[(size_t)ky * g.nw + kx / 32] |= 1u << (kx % 32);
+                if (first < 0) first = kx;
+                last = kx;
+            }
+        span[ky] = first < 0 ? make_int2(g.kwp, 0) : make_int2(first & ~3, (last + 4) & ~3);
+    }
+    return with_device_table(table, s, [&](void *d) {
+        const int2 *dspan = (const int2 *)d;
+        const uint32_t *dbits = (const uint32_t *)((const char *)d + span_bytes);
+        auto kern = focal_wide_kernel<kAllStats>;
+        switch (stat) {
+            case XRS_STAT_MEAN: kern = focal_wide_kernel<XRS_STAT_MEAN>; break;
+            case XRS_STAT_SUM: kern = focal_wide_kernel<XRS_STAT_SUM>; break;
+            case XRS_STAT_MIN: kern = focal_wide_kernel<XRS_STAT_MIN>; break;
+            case XRS_STAT_MAX: kern = focal_wide_kernel<XRS_STAT_MAX>; break;
+            case XRS_STAT_STD: kern = focal_wide_kernel<XRS_STAT_STD>; break;
+            case XRS_STAT_RANGE: kern = focal_wide_kernel<XRS_STAT_RANGE>; break;
+            case XRS_STAT_VAR: kern = focal_wide_kernel<XRS_STAT_VAR>; break;
+        }
+        return launch_wide(kern, g, s, stat == kAllStats ? kFocalWideFused : kFocalWide, in, dspan, dbits, planes,
+                           g);
+    });
+}
+
 static int check_common(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
                         const double *kernel, int kh, int kw) {
     XRS_REQUIRE(in && out && kernel, "NULL pointer");
     XRS_REQUIRE((const void *)in != (const void *)out, "in and out must not alias");
-    XRS_REQUIRE(kh >= 1 && kw >= 1 && (kh & 1) && (kw & 1), "kernel dimensions must be odd");
-    XRS_REQUIRE(kh * kw <= kMaxTaps && kh <= 63 && kw <= 63, "kernel too large (max 49x49 taps, 63 per side)");
+    if (const int rc = check_window(kh, kw)) return rc;
     XRS_REQUIRE(in_pitch % 4 == 0 && in_pitch >= W * 4 && out_pitch % 4 == 0 && out_pitch >= W * 4,
                 "pitches must be multiples of 4 bytes and >= row bytes");
     XRS_REQUIRE(H < (1LL << 31) - 64 && W < (1LL << 31) - 256, "raster dimension too large");
@@ -672,6 +1035,7 @@ int xrs_convolve2d_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
     if (H <= 0 || W <= 0) return XRS_OK;
     const int rc = check_common(in, in_pitch, out, out_pitch, H, W, kernel, kh, kw);
     if (rc) return rc;
+    if (is_wide(kh, kw)) return conv2d_wide(in, in_pitch, out, out_pitch, H, W, kernel, kh, kw, (cudaStream_t)s);
     if (kh == 3 && kw == 3) return xrs_conv3_strip(in, in_pitch, out, out_pitch, H, W, kernel, (cudaStream_t)s);
     {
         int brc = XRS_OK;
@@ -712,6 +1076,11 @@ int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
     const int rc = check_common(in, in_pitch, out, out_pitch, H, W, kernel, kh, kw);
     if (rc) return rc;
     XRS_REQUIRE(stat >= XRS_STAT_MEAN && stat <= XRS_STAT_VAR, "unknown focal statistic");
+    if (is_wide(kh, kw)) {
+        StatPlanes planes = {};
+        planes.p[stat] = out;
+        return focal_wide(in, in_pitch, planes, out_pitch, H, W, kernel, kh, kw, stat, (cudaStream_t)s);
+    }
     static thread_local MaskBits mask;
     bool all_ones = true;
     for (int i = 0; i < kh * kw; ++i) {
@@ -757,6 +1126,8 @@ int xrs_focal_stats_multi_f32(const float *in, int64_t in_pitch, float *out, int
         XRS_REQUIRE(planes.p[stats[i]] == nullptr, "statistic requested twice");
         planes.p[stats[i]] = reinterpret_cast<float *>(reinterpret_cast<char *>(out) + (int64_t)i * plane_stride);
     }
+    if (is_wide(kh, kw))
+        return focal_wide(in, in_pitch, planes, out_pitch, H, W, kernel, kh, kw, kAllStats, (cudaStream_t)s);
     TileGeom g;
     CUtensorMap tmap;
     if (n_stats >= 2 && tile_geom(g, &tmap, in, in_pitch, out, out_pitch, H, W, kh, kw, kTileH)) {

@@ -93,6 +93,7 @@ static int host_op_shape(int op, int in_dtype, const double *p, const double *au
         case XRS_OP_FOCAL_STAT:
             XRS_REQUIRE(in_dtype == XRS_F32, "convolve and focal statistics take float32 cells");
             XRS_REQUIRE(p && aux, "kernel parameters missing");
+            if (const int rc = check_window((int)p[0], (int)p[1])) return rc;
             sh->radius = (int)p[0] / 2;
             return XRS_OK;
     }
