@@ -331,6 +331,34 @@ def test_focal_stats_fused_equals_per_statistic_apply(xb, stats):
             assert_close_f32(got[i], ref, atol=atol, what=s)
 
 
+@pytest.mark.parametrize("stats", [["mean"], ["var"], ["sum", "min", "max"], STATS])
+def test_focal_stats_one_call_on_any_width(xb, stats, monkeypatch):
+    """On a device raster whose width is not a multiple of 4, and for a single statistic, focal_stats makes
+    one xrs_focal_stats_multi_f32 call and returns what stacking one `apply` per statistic returns."""
+    import pandas as pd
+    from xrspatial_b200 import _lib, focal
+    from xrspatial_b200._xr import concat
+    from xrspatial_b200.convolution import circle_kernel
+    rng = np.random.default_rng(17)
+    z = terrain(rng, 37, 131, nans=0.05)
+    agg = xb.DataArray(dev(z), dims=("y", "x"), coords={"y": np.arange(37)[::-1], "x": np.arange(131) * 2.0},
+                       attrs={"res": (1, 1), "crs": "x"}, name="dem")
+    real_call = _lib.call
+    for kern in (circle_kernel(1, 1, 2), np.ones((3, 3))):
+        want = concat([focal.apply(agg, kern, func=s) for s in stats], pd.Index(stats, name="stats", dtype=object))
+        calls = []
+        monkeypatch.setattr(_lib, "call", lambda name, *a: (calls.append(name), real_call(name, *a))[1])
+        got = focal.focal_stats(agg, kern, stats_funcs=stats)
+        monkeypatch.setattr(_lib, "call", real_call)
+        assert calls == ["xrs_focal_stats_multi_f32"]
+        assert got.dims == want.dims and got.name == want.name and got.attrs == want.attrs
+        assert list(got.coords) == list(want.coords)
+        for c in want.coords:
+            np.testing.assert_array_equal(np.asarray(got.coords[c]), np.asarray(want.coords[c]))
+        assert got.data.dtype == want.data.dtype and tuple(got.shape) == tuple(want.shape)
+        np.testing.assert_array_equal(host(got), host(want))
+
+
 def test_input_not_modified_and_metadata(xb):
     rng = np.random.default_rng(1)
     z = terrain(rng, 40, 64)

@@ -2,7 +2,7 @@
 
 conv2d_kernel / conv2d_fixed_kernel (128 x 64 output tiles), the 3 x 3 strip kernels and conv2d_direct_kernel all
 compute acc = fma(w, (double)x, acc) in row-major tap order from +0.0 with out-of-raster cells NaN, so they must
-agree bit for bit with each other and with the FMA oracle (oracle.convolve_2d_fma).  focal_stat_kernel (128 x 32
+agree bit for bit with each other and with the FMA oracle (oracle.convolve_2d_fma).  focal_tile_kernel (128 x 32
 tiles) and focal_stat_direct_kernel share Numba's nan-reducers, so mean, sum, min, max and range must agree bit
 for bit, sign bits included.  The running box (uniform convolve_2d and focal.apply mean over all-ones windows) is
 held to a per-window bound at planted magnitudes from 2^24 M to FLT_MAX.

@@ -3,8 +3,8 @@ than 63 cells on a side, up to 2047 x 2047.
 
 conv2d_wide_kernel must agree bit for bit with the FMA oracle (row-major fma(w, (double)x, acc) from +0.0 over
 every tap, out-of-raster taps NaN), and focal_wide_kernel with the oracle's Numba reducers for mean, sum, min,
-max and range (var and std within the bound of test_kxk_edges).  The fused kernel's planes must equal the
-single-statistic calls bit for bit.  The harness is test_kxk_edges's: the input inside a buffer of large
+max and range (var and std within the bound of test_kxk_edges).  The fused kernel's planes
+(focal_wide_kernel<kAllStats>) must equal the single-statistic calls bit for bit.  The harness is test_kxk_edges's: the input inside a buffer of large
 finite cells, the output inside a sentinel-filled pitched buffer, and an assert on the kernel that ran.  The
 oracle is O(taps) per cell, so the large windows run on small rasters.  Runs on an H100 (`-m gpu`)."""
 import ctypes

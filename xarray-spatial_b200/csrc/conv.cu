@@ -14,6 +14,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -44,36 +45,37 @@ struct TileGeom {
     size_t smem_bytes() const { return tile_cells() * sizeof(float) + 16; }   // the tile, then its mbarrier
 };
 
-// The tiled kernels' shared memory: the (tile + halo) block, then one mbarrier.  Thread 0 prefetches the
-// tensor-map descriptor and initialises the barrier; every thread returns after the CTA barrier.
-struct SmemTile {
-    float *tile32;
-    uint64_t *bar;
-};
-__device__ __forceinline__ SmemTile tile_preamble(const CUtensorMap *tmap, const TileGeom &g) {
+// The persistent loop of the tiled kernels over kTileW x tile_h output tiles: CTA b takes tiles b, b + gridDim.x,
+// ..., brings each (tile + halo) block into shared memory and runs body(tile32, x0, y0) on it.  Shared memory
+// holds the block, then one mbarrier; thread 0 initialises the barrier and issues the TMA boxes, everyone waits
+// on it.
+template <typename F>
+__device__ __forceinline__ void tile_loop(const CUtensorMap *tmap, const TileGeom &g, int tile_h, F &&body) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    SmemTile s;
-    s.tile32 = reinterpret_cast<float *>(smem_raw);
-    s.bar = reinterpret_cast<uint64_t *>(smem_raw + g.tile_cells() * sizeof(float));
+    float *tile32 = reinterpret_cast<float *>(smem_raw);
+    uint64_t *bar = reinterpret_cast<uint64_t *>(smem_raw + g.tile_cells() * sizeof(float));
     if (threadIdx.x == 0) {
         tma_prefetch_desc(tmap);
-        mbar_init(s.bar, 1);
+        mbar_init(bar, 1);
         mbar_fence_init();
     }
     __syncthreads();
-    return s;
-}
-
-__device__ __forceinline__ void load_tile_tma(const CUtensorMap *tmap, float *tile32, uint64_t *bar,
-                                              const TileGeom &g, int tx0, int ty0, uint32_t parity) {
-    // one elected thread issues the boxes; everyone waits on the mbarrier
-    if (threadIdx.x == 0) {
-        const int nbox = (g.sh + g.box_h - 1) / g.box_h;
-        mbar_arrive_expect_tx(bar, (uint32_t)(nbox * g.box_h * g.sw * sizeof(float)));
-        for (int b = 0; b < nbox; ++b)
-            tma_load_2d(tile32 + (size_t)b * g.box_h * g.sw, tmap, bar, tx0 - g.pad, ty0 - g.ry + b * g.box_h);
+    const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
+    uint32_t parity = 0;
+    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const int tile_y = (int)(t / g.tiles_x), tile_x = (int)(t % g.tiles_x);
+        const int x0 = tile_x * kTileW, y0 = tile_y * tile_h;
+        if (threadIdx.x == 0) {
+            const int nbox = (g.sh + g.box_h - 1) / g.box_h;
+            mbar_arrive_expect_tx(bar, (uint32_t)(nbox * g.box_h * g.sw * sizeof(float)));
+            for (int b = 0; b < nbox; ++b)
+                tma_load_2d(tile32 + (size_t)b * g.box_h * g.sw, tmap, bar, x0 - g.pad, y0 - g.ry + b * g.box_h);
+        }
+        mbar_wait(bar, parity);
+        parity ^= 1u;
+        body(tile32, x0, y0);
+        __syncthreads();  // the tile buffer is reused by the next iteration
     }
-    mbar_wait(bar, parity);
 }
 
 // ----------------------------------------------------------------------------- convolve
@@ -84,23 +86,33 @@ __device__ __forceinline__ void load_tile_tma(const CUtensorMap *tmap, float *ti
 // accumulators per thread give the FP64 pipe enough parallelism at 2-3 CTAs per SM.
 constexpr int kConvTileH = 64;
 
+// A thread's 4 x 8 outputs: rows y .. y + 3, columns xa .. xa + 3 and xa + 64 .. xa + 67.
+__device__ __forceinline__ void store_tile32(float *out, int64_t pitch_elems, const TileGeom &g, int64_t y,
+                                             int64_t xa, const double (&acc)[4][8]) {
+    const int64_t xb = xa + 64;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int64_t yo = y + r;
+        if (yo < g.H) {  // W % 4 == 0 on this path: a float4 is all-in or all-out
+            float *orow = out + yo * pitch_elems;
+            if (xa < g.W)
+                __stcs(reinterpret_cast<float4 *>(orow + xa),
+                       make_float4((float)acc[r][0], (float)acc[r][1], (float)acc[r][2], (float)acc[r][3]));
+            if (xb < g.W)
+                __stcs(reinterpret_cast<float4 *>(orow + xb),
+                       make_float4((float)acc[r][4], (float)acc[r][5], (float)acc[r][6], (float)acc[r][7]));
+        }
+    }
+}
+
 // KW > 0: kernel width known at compile time (5, 7, 9: the usual custom kernels) -- the tap-chunk
 // loop unrolls and its chunk / tap tests fold away; KW == 0: any odd shape.
 template <int KW>
 __global__ void __launch_bounds__(256)
 conv2d_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ ConvWeights cw,
               float *__restrict__ out, int64_t out_pitch_elems, const TileGeom g) {
-    const auto [tile32, bar] = tile_preamble(&tmap, g);
-
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
-    uint32_t parity = 0;
-    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        const int tile_y = (int)(t / g.tiles_x), tile_x = (int)(t % g.tiles_x);
-        const int x0 = tile_x * kTileW, y0 = tile_y * kConvTileH;
-        load_tile_tma(&tmap, tile32, bar, g, x0, y0, parity);
-        parity ^= 1u;
-
+    tile_loop(&tmap, g, kConvTileH, [&](const float *tile32, int x0, int y0) {
         double acc[4][8];
 #pragma unroll
         for (int r = 0; r < 4; ++r)
@@ -191,22 +203,8 @@ conv2d_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ 
                 for (int kb = 0; kb < n_taps; kb += 4) chunk(kb);
             }
         }
-        const int64_t xa = (int64_t)x0 + 4 * tx, xb = xa + 64;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int64_t yo = (int64_t)y0 + ty * 4 + r;
-            if (yo < g.H) {  // W % 4 == 0 on this path: a float4 is all-in or all-out
-                float *orow = out + yo * out_pitch_elems;
-                if (xa < g.W)
-                    __stcs(reinterpret_cast<float4 *>(orow + xa),
-                           make_float4((float)acc[r][0], (float)acc[r][1], (float)acc[r][2], (float)acc[r][3]));
-                if (xb < g.W)
-                    __stcs(reinterpret_cast<float4 *>(orow + xb),
-                           make_float4((float)acc[r][4], (float)acc[r][5], (float)acc[r][6], (float)acc[r][7]));
-            }
-        }
-        __syncthreads();  // the tile buffer is reused by the next iteration
-    }
+        store_tile32(out, out_pitch_elems, g, (int64_t)y0 + ty * 4, (int64_t)x0 + 4 * tx, acc);
+    });
 }
 
 // Square K x K kernels with K in {5, 7, ..., 13} (the usual hand-made filters; at K = 15 the
@@ -220,15 +218,8 @@ conv2d_fixed_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_const
                     float *__restrict__ out, int64_t out_pitch_elems, const TileGeom g) {
     constexpr int kOff = (K / 2 + 3) / 4 * 4 - K / 2;   // column of tap 0 relative to the aligned origin
     constexpr int kVals = (kOff + K + 3 + 3) / 4 * 4;   // cells a thread needs per row and half
-    const auto [tile32, bar] = tile_preamble(&tmap, g);
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
-    uint32_t parity = 0;
-    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        const int tile_y = (int)(t / g.tiles_x), tile_x = (int)(t % g.tiles_x);
-        const int x0 = tile_x * kTileW, y0 = tile_y * kConvTileH;
-        load_tile_tma(&tmap, tile32, bar, g, x0, y0, parity);
-        parity ^= 1u;
+    tile_loop(&tmap, g, kConvTileH, [&](const float *tile32, int x0, int y0) {
         double acc[4][8];
 #pragma unroll
         for (int r = 0; r < 4; ++r)
@@ -262,22 +253,8 @@ conv2d_fixed_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_const
                 }
             }
         }
-        const int64_t xa = (int64_t)x0 + 4 * tx, xb = xa + 64;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int64_t yo = (int64_t)y0 + ty * 4 + r;
-            if (yo < g.H) {
-                float *orow = out + yo * out_pitch_elems;
-                if (xa < g.W)
-                    __stcs(reinterpret_cast<float4 *>(orow + xa),
-                           make_float4((float)acc[r][0], (float)acc[r][1], (float)acc[r][2], (float)acc[r][3]));
-                if (xb < g.W)
-                    __stcs(reinterpret_cast<float4 *>(orow + xb),
-                           make_float4((float)acc[r][4], (float)acc[r][5], (float)acc[r][6], (float)acc[r][7]));
-            }
-        }
-        __syncthreads();
-    }
+        store_tile32(out, out_pitch_elems, g, (int64_t)y0 + ty * 4, (int64_t)x0 + 4 * tx, acc);
+    });
 }
 
 // Fallback for rasters TMA cannot describe: one thread per cell, bounds-checked loads.
@@ -358,10 +335,6 @@ __device__ __forceinline__ float focal_reduce(const Fetch &fetch, const MaskBits
     }
 }
 
-// Register-blocked like conv2d_kernel: a thread owns 4 x 4 outputs, walks the input rows of its
-// window once (twice for var / std), loads 8 cells per 4-tap chunk with two LDS.128 and feeds
-// every (output row, tap) pair whose mask bit is set.  Taps are visited in row-major window
-// order for each output, so the float32 `sum` is bit-identical to np.nansum on the scratch.
 // One loaded window cell as the reducers see it: NaN test, f64 widening and the "skip NaN" masking
 // happen once per loaded cell, not once per (output, tap) use.
 struct FocalCell {
@@ -373,6 +346,136 @@ struct FocalCell {
     bool ok;
 };
 
+// The 8 cells of a 4-tap chunk: two 16-byte loads from p.
+__device__ __forceinline__ void load_cells(const float *p, FocalCell (&cell)[8]) {
+    const float4 q0 = *reinterpret_cast<const float4 *>(p);
+    const float4 q1 = *reinterpret_cast<const float4 *>(p + 4);
+    const float v[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        cell[i].v = v[i];
+        cell[i].ok = (v[i] == v[i]);
+        cell[i].vz = cell[i].ok ? v[i] : 0.f;
+        cell[i].d = (double)v[i];
+        cell[i].dz = (double)cell[i].vz;
+        cell[i].one = cell[i].ok ? 1 : 0;
+    }
+}
+
+// The output planes of the focal statistics.
+struct StatPlanes {
+    float *p[7];  // indexed by xrs_focal_stat; nullptr = not requested
+};
+constexpr int kAllStats = -1;  // as a kernel's statistic: every statistic whose plane is set
+
+// The tiled kernel's output: the plane of its one statistic, or every plane for kAllStats.
+template <int STAT>
+using FocalOut = std::conditional_t<STAT == kAllStats, StatPlanes, float *__restrict__>;
+template <int STAT>
+FocalOut<STAT> focal_out(const StatPlanes &planes) {
+    if constexpr (STAT == kAllStats) return planes;
+    else return planes.p[STAT];
+}
+__device__ __forceinline__ float *plane_of(const StatPlanes &out, int s) { return out.p[s]; }
+__device__ __forceinline__ float *plane_of(float *out, int) { return out; }
+
+// The statistics of a thread's 4 x 4 outputs, for the tiled and the wide kernels alike.  STAT is one
+// xrs_focal_stat, or kAllStats for every statistic whose plane in `out` is set.  sweep(f) calls f(r, c, cell) for
+// every window cell of output (r, c), in row-major window order; store(plane, res) writes 4 x 4 results.
+// Sweep A accumulates the float64 sum and the count (mean, var, std) and the float32 row-major sum (sum); sweep B
+// the squared deviations about the float64 mean (var, std).  min and max (min, max, range) go into sweep A when
+// kMinMaxInA, into sweep B otherwise: which is cheaper depends on the memory path.  A sweep with nothing to
+// accumulate does not run: for one statistic that is known at compile time, for kAllStats the planes decide.
+template <int STAT, bool kMinMaxInA, typename Out, typename Sweep, typename Store>
+__device__ __forceinline__ void focal_outputs(const Out &out, const Sweep &sweep, const Store &store) {
+    constexpr bool kAll = STAT == kAllStats;
+    constexpr bool kMean = kAll || STAT == XRS_STAT_MEAN || STAT == XRS_STAT_VAR || STAT == XRS_STAT_STD;
+    constexpr bool kSum = kAll || STAT == XRS_STAT_SUM;
+    constexpr bool kMinMax = kAll || STAT == XRS_STAT_MIN || STAT == XRS_STAT_MAX || STAT == XRS_STAT_RANGE;
+    constexpr bool kSsd = kAll || STAT == XRS_STAT_VAR || STAT == XRS_STAT_STD;
+    auto want = [&](int s) { return kAll ? plane_of(out, s) != nullptr : STAT == s; };
+    float res[4][4];
+    double mean[4][4];
+    int cnt[4][4];
+    float fsum[4][4], mn[4][4], mx[4][4];
+    double ssd[4][4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+            mean[r][c] = 0.0, cnt[r][c] = 0, fsum[r][c] = 0.f, mn[r][c] = mx[r][c] = nan_of<float>();
+    auto min_max = [&](int r, int c, const FocalCell &q) {
+        nan_min_step(mn[r][c], q.v);
+        nan_max_step(mx[r][c], q.v);
+    };
+    auto store_min_max = [&] {
+        if (want(XRS_STAT_MIN)) store(plane_of(out, XRS_STAT_MIN), mn);
+        if (want(XRS_STAT_MAX)) store(plane_of(out, XRS_STAT_MAX), mx);
+        if (want(XRS_STAT_RANGE)) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) res[r][c] = mx[r][c] - mn[r][c];
+            store(plane_of(out, XRS_STAT_RANGE), res);
+        }
+    };
+    if constexpr (kMean || kSum || (kMinMaxInA && kMinMax))
+        sweep([&](int r, int c, const FocalCell &q) {  // sweep A
+            if (kMean) mean[r][c] += q.dz, cnt[r][c] += q.one;
+            if (kSum) fsum[r][c] += q.vz;
+            if (kMinMaxInA && kMinMax) min_max(r, c, q);
+        });
+    if (want(XRS_STAT_SUM)) store(plane_of(out, XRS_STAT_SUM), fsum);
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            mean[r][c] = mean[r][c] / (double)cnt[r][c];
+            res[r][c] = (float)mean[r][c];
+        }
+    if (want(XRS_STAT_MEAN)) store(plane_of(out, XRS_STAT_MEAN), res);
+    if constexpr (kMinMaxInA) store_min_max();
+    constexpr bool kMinMaxInB = !kMinMaxInA && kMinMax;
+    if constexpr (kSsd || kMinMaxInB) {
+        if ((kMinMaxInB && (want(XRS_STAT_MIN) || want(XRS_STAT_MAX) || want(XRS_STAT_RANGE))) || want(XRS_STAT_VAR) ||
+            want(XRS_STAT_STD)) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) ssd[r][c] = 0.0;
+            sweep([&](int r, int c, const FocalCell &q) {  // sweep B
+                if (kSsd) {
+                    const double d = q.d - mean[r][c];
+                    ssd[r][c] += q.ok ? d * d : 0.0;
+                }
+                if (kMinMaxInB) min_max(r, c, q);
+            });
+            if constexpr (kMinMaxInB) store_min_max();
+            if (want(XRS_STAT_VAR) || want(XRS_STAT_STD)) {
+#pragma unroll
+                for (int r = 0; r < 4; ++r)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        ssd[r][c] = ssd[r][c] / (double)cnt[r][c];
+                        res[r][c] = (float)ssd[r][c];
+                    }
+                if (want(XRS_STAT_VAR)) store(plane_of(out, XRS_STAT_VAR), res);
+                if (want(XRS_STAT_STD)) {
+#pragma unroll
+                    for (int r = 0; r < 4; ++r)
+#pragma unroll
+                        for (int c = 0; c < 4; ++c) res[r][c] = (float)sqrt(ssd[r][c]);
+                    store(plane_of(out, XRS_STAT_STD), res);
+                }
+            }
+        }
+    }
+}
+
+// Register-blocked like conv2d_kernel: a thread owns 4 x 4 outputs, walks the input rows of its
+// window once per sweep, loads 8 cells per 4-tap chunk with two LDS.128 and feeds every (output row,
+// tap) pair whose mask bit is set.  Taps are visited in row-major window order for each output, so
+// the float32 `sum` is bit-identical to np.nansum on the scratch.
 template <typename F>
 __device__ __forceinline__ void focal_sweep(const float *tile32, const MaskBits &mask, const TileGeom &g, int tx,
                                             int ty, F &&f) {
@@ -381,19 +484,8 @@ __device__ __forceinline__ void focal_sweep(const float *tile32, const MaskBits 
     for (int j = 0; j < rows_in; ++j) {
         const float *rowp = tile32 + (size_t)(ty * 4 + j) * g.sw + 4 * tx;
         for (int kb = 0; kb < n_taps; kb += 4) {
-            const float4 q0 = *reinterpret_cast<const float4 *>(rowp + kb);
-            const float4 q1 = *reinterpret_cast<const float4 *>(rowp + kb + 4);
-            const float v[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
             FocalCell cell[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                cell[i].v = v[i];
-                cell[i].ok = (v[i] == v[i]);
-                cell[i].vz = cell[i].ok ? v[i] : 0.f;
-                cell[i].d = (double)v[i];
-                cell[i].dz = (double)cell[i].vz;
-                cell[i].one = cell[i].ok ? 1 : 0;
-            }
+            load_cells(rowp + kb, cell);
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
                 const int ky = j - r;
@@ -412,99 +504,6 @@ __device__ __forceinline__ void focal_sweep(const float *tile32, const MaskBits 
     }
 }
 
-template <int STAT>
-__global__ void __launch_bounds__(256)
-focal_stat_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ MaskBits mask,
-                  float *__restrict__ out, int64_t out_pitch_elems, const TileGeom g) {
-    const auto [tile32, bar] = tile_preamble(&tmap, g);
-    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-    const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
-    uint32_t parity = 0;
-    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        const int tile_y = (int)(t / g.tiles_x), tile_x = (int)(t % g.tiles_x);
-        const int x0 = tile_x * kTileW, y0 = tile_y * kTileH;
-        load_tile_tma(&tmap, tile32, bar, g, x0, y0, parity);
-        parity ^= 1u;
-        float res[4][4];
-        if constexpr (STAT == XRS_STAT_MEAN || STAT == XRS_STAT_VAR || STAT == XRS_STAT_STD) {
-            double sum[4][4];
-            int cnt[4][4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) sum[r][c] = 0.0, cnt[r][c] = 0;
-            focal_sweep(tile32, mask, g, tx, ty, [&](int r, int c, const FocalCell &q) {
-                sum[r][c] += q.dz;
-                cnt[r][c] += q.one;
-            });
-            if constexpr (STAT == XRS_STAT_MEAN) {
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) res[r][c] = (float)(sum[r][c] / (double)cnt[r][c]);
-            } else {
-                double ssd[4][4];
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) sum[r][c] = sum[r][c] / (double)cnt[r][c], ssd[r][c] = 0.0;
-                focal_sweep(tile32, mask, g, tx, ty, [&](int r, int c, const FocalCell &q) {
-                    const double d = q.d - sum[r][c];
-                    ssd[r][c] += q.ok ? d * d : 0.0;
-                });
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        const double var = ssd[r][c] / (double)cnt[r][c];
-                        res[r][c] = (float)(STAT == XRS_STAT_VAR ? var : sqrt(var));
-                    }
-            }
-        } else if constexpr (STAT == XRS_STAT_SUM) {
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) res[r][c] = 0.f;
-            focal_sweep(tile32, mask, g, tx, ty, [&](int r, int c, const FocalCell &q) { res[r][c] += q.vz; });
-        } else {
-            float mn[4][4], mx[4][4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) mn[r][c] = mx[r][c] = nan_of<float>();
-            focal_sweep(tile32, mask, g, tx, ty, [&](int r, int c, const FocalCell &q) {
-                nan_min_step(mn[r][c], q.v);
-                nan_max_step(mx[r][c], q.v);
-            });
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c)
-                    res[r][c] = STAT == XRS_STAT_MIN ? mn[r][c] : STAT == XRS_STAT_MAX ? mx[r][c] : mx[r][c] - mn[r][c];
-        }
-        const int64_t xo = (int64_t)x0 + 4 * tx;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int64_t yo = (int64_t)y0 + ty * 4 + r;
-            if (yo < g.H && xo < g.W)  // W % 4 == 0 on this path
-                __stcs(reinterpret_cast<float4 *>(out + yo * out_pitch_elems + xo),
-                       make_float4(res[r][0], res[r][1], res[r][2], res[r][3]));
-        }
-        __syncthreads();
-    }
-}
-
-// All requested statistics of one window in ONE pass over the raster (focal.focal_stats,
-// focal.py:800-878, is seven `apply` calls stacked with xr.concat): the tile is loaded once,
-// sweep A accumulates the float64 sum, the count and the float32 row-major sum of every output's
-// window, sweep B the min / max and the squared deviations about the float64 mean, and each
-// statistic goes straight into its plane of the (stats, y, x) result -- 2 sweeps and one tile
-// load instead of 9 and 7, and no stacking copy.  Per-statistic arithmetic is the single-stat
-// kernel's, operation for operation.
-struct StatPlanes {
-    float *p[7];  // indexed by xrs_focal_stat; nullptr = not requested
-};
-
 __device__ __forceinline__ void store_tile16(float *plane, int64_t pitch_elems, int64_t H, int64_t W, int64_t y0,
                                              int64_t xo, const float (&res)[4][4]) {
 #pragma unroll
@@ -514,87 +513,31 @@ __device__ __forceinline__ void store_tile16(float *plane, int64_t pitch_elems, 
                    make_float4(res[r][0], res[r][1], res[r][2], res[r][3]));
 }
 
-__global__ void __launch_bounds__(256, 2)
-focal_stats_multi_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ MaskBits mask,
-                         const StatPlanes planes, int64_t out_pitch_elems, const TileGeom g) {
-    const auto [tile32, bar] = tile_preamble(&tmap, g);
-    const bool want_b = planes.p[XRS_STAT_MIN] || planes.p[XRS_STAT_MAX] || planes.p[XRS_STAT_RANGE] ||
-                        planes.p[XRS_STAT_STD] || planes.p[XRS_STAT_VAR];
-    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-    const int64_t n_tiles = (int64_t)g.tiles_x * g.tiles_y;
-    uint32_t parity = 0;
-    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        const int tile_y = (int)(t / g.tiles_x), tile_x = (int)(t % g.tiles_x);
-        const int x0 = tile_x * kTileW, y0 = tile_y * kTileH;
-        load_tile_tma(&tmap, tile32, bar, g, x0, y0, parity);
-        parity ^= 1u;
-        const int64_t xo = (int64_t)x0 + 4 * tx, yo = (int64_t)y0 + ty * 4;
-        float res[4][4];
-        double mean[4][4];
-        int cnt[4][4];
-        {
-            float fsum[4][4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) mean[r][c] = 0.0, cnt[r][c] = 0, fsum[r][c] = 0.f;
-            focal_sweep(tile32, mask, g, tx, ty, [&](int r, int c, const FocalCell &q) {
-                mean[r][c] += q.dz;
-                cnt[r][c] += q.one;
-                fsum[r][c] += q.vz;
+// One statistic, or (kAllStats) every requested statistic in ONE pass over the raster: focal.focal_stats
+// (focal.py:800-878) is seven `apply` calls stacked with xr.concat; here the tile is loaded once, the fused
+// kernel runs 2 sweeps instead of 9, and each statistic goes straight into its plane of the (stats, y, x)
+// result, with no stacking copy.  min and max are accumulated in sweep B.
+template <int STAT>
+__global__ void __launch_bounds__(256, STAT == kAllStats ? 2 : 0)
+focal_tile_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ MaskBits mask,
+                  const FocalOut<STAT> out, int64_t out_pitch_elems, const TileGeom g) {
+    tile_loop(&tmap, g, kTileH, [&](const float *tile32, int x0, int y0) {
+        const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+        auto sweep = [&](auto &&f) { focal_sweep(tile32, mask, g, tx, ty, f); };
+        // Where the store coordinates are computed steers register allocation: before the sweeps the fused kernel
+        // runs about 2 % faster, after them the single-statistic kernels need up to 6 fewer registers.
+        if constexpr (STAT == kAllStats) {
+            const int64_t xo = (int64_t)x0 + 4 * tx, yo = (int64_t)y0 + ty * 4;
+            focal_outputs<STAT, false>(out, sweep, [&](float *plane, const float (&res)[4][4]) {
+                store_tile16(plane, out_pitch_elems, g.H, g.W, yo, xo, res);
             });
-            if (planes.p[XRS_STAT_SUM]) store_tile16(planes.p[XRS_STAT_SUM], out_pitch_elems, g.H, g.W, yo, xo, fsum);
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    mean[r][c] = mean[r][c] / (double)cnt[r][c];
-                    res[r][c] = (float)mean[r][c];
-                }
-            if (planes.p[XRS_STAT_MEAN]) store_tile16(planes.p[XRS_STAT_MEAN], out_pitch_elems, g.H, g.W, yo, xo, res);
-        }
-        if (want_b) {
-            float mn[4][4], mx[4][4];
-            double ssd[4][4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) mn[r][c] = mx[r][c] = nan_of<float>(), ssd[r][c] = 0.0;
-            focal_sweep(tile32, mask, g, tx, ty, [&](int r, int c, const FocalCell &q) {
-                const double d = q.d - mean[r][c];
-                ssd[r][c] += q.ok ? d * d : 0.0;
-                nan_min_step(mn[r][c], q.v);
-                nan_max_step(mx[r][c], q.v);
+        } else {
+            focal_outputs<STAT, false>(out, sweep, [&](float *plane, const float (&res)[4][4]) {
+                const int64_t xo = (int64_t)x0 + 4 * tx, yo = (int64_t)y0 + ty * 4;
+                store_tile16(plane, out_pitch_elems, g.H, g.W, yo, xo, res);
             });
-            if (planes.p[XRS_STAT_MIN]) store_tile16(planes.p[XRS_STAT_MIN], out_pitch_elems, g.H, g.W, yo, xo, mn);
-            if (planes.p[XRS_STAT_MAX]) store_tile16(planes.p[XRS_STAT_MAX], out_pitch_elems, g.H, g.W, yo, xo, mx);
-            if (planes.p[XRS_STAT_RANGE]) {
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) res[r][c] = mx[r][c] - mn[r][c];
-                store_tile16(planes.p[XRS_STAT_RANGE], out_pitch_elems, g.H, g.W, yo, xo, res);
-            }
-            if (planes.p[XRS_STAT_VAR] || planes.p[XRS_STAT_STD]) {
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        ssd[r][c] = ssd[r][c] / (double)cnt[r][c];
-                        res[r][c] = (float)ssd[r][c];
-                    }
-                if (planes.p[XRS_STAT_VAR]) store_tile16(planes.p[XRS_STAT_VAR], out_pitch_elems, g.H, g.W, yo, xo, res);
-                if (planes.p[XRS_STAT_STD]) {
-#pragma unroll
-                    for (int r = 0; r < 4; ++r)
-#pragma unroll
-                        for (int c = 0; c < 4; ++c) res[r][c] = (float)sqrt(ssd[r][c]);
-                    store_tile16(planes.p[XRS_STAT_STD], out_pitch_elems, g.H, g.W, yo, xo, res);
-                }
-            }
         }
-        __syncthreads();
-    }
+    });
 }
 
 __global__ void __launch_bounds__(256)
@@ -625,7 +568,6 @@ focal_stat_direct_kernel(const float *__restrict__ in, int64_t in_pitch_elems, c
 // its ones and a bit row) live in a stream-ordered device buffer made for the call.
 constexpr int kWideSide = 2047;
 constexpr int kWideConvW = 2048, kWideStatW = 1024, kRing = 4;
-constexpr int kAllStats = -1;  // focal_wide_kernel: every statistic whose plane is set
 
 struct WideGeom {
     int64_t H, W, in_pitch, out_pitch;  // pitches in cells
@@ -742,22 +684,14 @@ conv2d_wide_kernel(const float *__restrict__ in, const double *__restrict__ w, f
     }
 }
 
-// The statistics of focal_stat_kernel / focal_stats_multi_kernel, operation for operation, over a thread's
-// 4 x 4 outputs (columns base .. base + 3).  Sweep A: float64 sum, count, float32 sum, min and max; sweep B,
-// only for var / std: the squared deviations about the float64 mean.  STAT is one xrs_focal_stat (one output
-// plane), or kAllStats for every plane that is set.  Each sweep visits, per input row, only the 4-tap chunks inside
+// The statistics of focal_tile_kernel over a wide window (focal_outputs, with min and max in sweep A), a thread's
+// 4 x 4 outputs being columns base .. base + 3.  Each sweep visits, per input row, only the 4-tap chunks inside
 // the union of the spans of ones of the (up to four) kernel rows it feeds.
 template <int STAT>
 __global__ void __launch_bounds__(256)
 focal_wide_kernel(const float *__restrict__ in, const int2 *__restrict__ span, const uint32_t *__restrict__ bits,
                   const StatPlanes planes, const WideGeom g) {
     extern __shared__ __align__(16) float ring[];
-    auto want = [&](int s) { return STAT == kAllStats ? planes.p[s] != nullptr : STAT == s; };
-    // what sweep A accumulates: everything for the fused kernel, only what its statistic needs otherwise
-    constexpr bool kSums = STAT == kAllStats || STAT == XRS_STAT_MEAN || STAT == XRS_STAT_SUM ||
-                           STAT == XRS_STAT_VAR || STAT == XRS_STAT_STD;
-    constexpr bool kMinMax = STAT == kAllStats || STAT == XRS_STAT_MIN || STAT == XRS_STAT_MAX ||
-                             STAT == XRS_STAT_RANGE;
     const int base = 4 * threadIdx.x;
     for (int64_t t = blockIdx.x; t < g.n_tiles; t += gridDim.x) {
         const int64_t y0 = t / g.tiles_x * 4, x0 = t % g.tiles_x * kWideStatW, xs = x0 - g.kw / 2;
@@ -775,6 +709,8 @@ focal_wide_kernel(const float *__restrict__ in, const int2 *__restrict__ span, c
                     }
                 }
                 for (int kb = lo; kb < hi; kb += 4) {
+                    // load_cells written out: through the function, the compiler allocates this kernel's registers
+                    // differently and the fused and var / std instantiations need 2 more
                     const float4 q0 = *reinterpret_cast<const float4 *>(rowp + kb);
                     const float4 q1 = *reinterpret_cast<const float4 *>(rowp + kb + 4);
                     const float v[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
@@ -809,79 +745,14 @@ focal_wide_kernel(const float *__restrict__ in, const int2 *__restrict__ span, c
                 }
             });
         };
-        auto store = [&](int s, const float (&res)[4][4]) {
-            float *plane = planes.p[s];
+        focal_outputs<STAT, true>(planes, sweep, [&](float *plane, const float (&res)[4][4]) {
 #pragma unroll
             for (int r = 0; r < 4; ++r)
                 if (y0 + r < g.H)
 #pragma unroll
                     for (int c = 0; c < 4; ++c)
                         if (x0 + base + c < g.W) plane[(y0 + r) * g.out_pitch + x0 + base + c] = res[r][c];
-        };
-        float res[4][4];
-        double mean[4][4];
-        int cnt[4][4];
-        float fsum[4][4], mn[4][4], mx[4][4];
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-#pragma unroll
-            for (int c = 0; c < 4; ++c)
-                mean[r][c] = 0.0, cnt[r][c] = 0, fsum[r][c] = 0.f, mn[r][c] = mx[r][c] = nan_of<float>();
-        sweep([&](int r, int c, const FocalCell &q) {
-            if (kSums) {
-                mean[r][c] += q.dz;
-                cnt[r][c] += q.one;
-                fsum[r][c] += q.vz;
-            }
-            if (kMinMax) {
-                nan_min_step(mn[r][c], q.v);
-                nan_max_step(mx[r][c], q.v);
-            }
         });
-        if (want(XRS_STAT_SUM)) store(XRS_STAT_SUM, fsum);
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                mean[r][c] = mean[r][c] / (double)cnt[r][c];
-                res[r][c] = (float)mean[r][c];
-            }
-        if (want(XRS_STAT_MEAN)) store(XRS_STAT_MEAN, res);
-        if (want(XRS_STAT_MIN)) store(XRS_STAT_MIN, mn);
-        if (want(XRS_STAT_MAX)) store(XRS_STAT_MAX, mx);
-        if (want(XRS_STAT_RANGE)) {
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) res[r][c] = mx[r][c] - mn[r][c];
-            store(XRS_STAT_RANGE, res);
-        }
-        if (want(XRS_STAT_VAR) || want(XRS_STAT_STD)) {
-            double ssd[4][4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) ssd[r][c] = 0.0;
-            sweep([&](int r, int c, const FocalCell &q) {
-                const double d = q.d - mean[r][c];
-                ssd[r][c] += q.ok ? d * d : 0.0;
-            });
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    ssd[r][c] = ssd[r][c] / (double)cnt[r][c];
-                    res[r][c] = (float)ssd[r][c];
-                }
-            if (want(XRS_STAT_VAR)) store(XRS_STAT_VAR, res);
-            if (want(XRS_STAT_STD)) {
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) res[r][c] = (float)sqrt(ssd[r][c]);
-                store(XRS_STAT_STD, res);
-            }
-        }
     }
 }
 
@@ -937,6 +808,21 @@ static int conv2d_wide(const float *in, int64_t in_pitch, float *out, int64_t ou
     });
 }
 
+// Calls f(std::integral_constant<int, S>{}) with S = stat: one xrs_focal_stat, or kAllStats.
+template <typename F>
+static int with_stat(int stat, F &&f) {
+    switch (stat) {
+        case XRS_STAT_MEAN: return f(std::integral_constant<int, XRS_STAT_MEAN>{});
+        case XRS_STAT_SUM: return f(std::integral_constant<int, XRS_STAT_SUM>{});
+        case XRS_STAT_MIN: return f(std::integral_constant<int, XRS_STAT_MIN>{});
+        case XRS_STAT_MAX: return f(std::integral_constant<int, XRS_STAT_MAX>{});
+        case XRS_STAT_STD: return f(std::integral_constant<int, XRS_STAT_STD>{});
+        case XRS_STAT_RANGE: return f(std::integral_constant<int, XRS_STAT_RANGE>{});
+        case XRS_STAT_VAR: return f(std::integral_constant<int, XRS_STAT_VAR>{});
+        default: return f(std::integral_constant<int, kAllStats>{});
+    }
+}
+
 // stat: one xrs_focal_stat into planes.p[stat], or kAllStats
 static int focal_wide(const float *in, int64_t in_pitch, const StatPlanes &planes, int64_t out_pitch, int64_t H,
                       int64_t W, const double *kernel, int kh, int kw, int stat, cudaStream_t s) {
@@ -960,19 +846,22 @@ static int focal_wide(const float *in, int64_t in_pitch, const StatPlanes &plane
     return with_device_table(table, s, [&](void *d) {
         const int2 *dspan = (const int2 *)d;
         const uint32_t *dbits = (const uint32_t *)((const char *)d + span_bytes);
-        auto kern = focal_wide_kernel<kAllStats>;
-        switch (stat) {
-            case XRS_STAT_MEAN: kern = focal_wide_kernel<XRS_STAT_MEAN>; break;
-            case XRS_STAT_SUM: kern = focal_wide_kernel<XRS_STAT_SUM>; break;
-            case XRS_STAT_MIN: kern = focal_wide_kernel<XRS_STAT_MIN>; break;
-            case XRS_STAT_MAX: kern = focal_wide_kernel<XRS_STAT_MAX>; break;
-            case XRS_STAT_STD: kern = focal_wide_kernel<XRS_STAT_STD>; break;
-            case XRS_STAT_RANGE: kern = focal_wide_kernel<XRS_STAT_RANGE>; break;
-            case XRS_STAT_VAR: kern = focal_wide_kernel<XRS_STAT_VAR>; break;
-        }
-        return launch_wide(kern, g, s, stat == kAllStats ? kFocalWideFused : kFocalWide, in, dspan, dbits, planes,
-                           g);
+        return with_stat(stat, [&](auto S) {
+            return launch_wide(focal_wide_kernel<S>, g, s, S == kAllStats ? kFocalWideFused : kFocalWide, in, dspan,
+                               dbits, planes, g);
+        });
     });
+}
+
+// The tiled and bounds-checked kernels' mask (focal.py:323: the cells where the kernel is 1); returns whether the
+// window is all ones.
+static bool mask_bits(MaskBits &mask, const double *kernel, int kh, int kw) {
+    bool all_ones = true;
+    for (int i = 0; i < kh * kw; ++i) {
+        mask.m[i] = (kernel[i] == 1.0) ? 1 : 0;
+        all_ones = all_ones && mask.m[i];
+    }
+    return all_ones;
 }
 
 static int check_common(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
@@ -1026,6 +915,40 @@ bool try_box_stream(const float *in, int64_t in_pitch, float *out, int64_t out_p
 // box_stream.cu, NaN-skipping mode: focal.apply mean over an all-ones window
 bool try_box_nanmean(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
                      int kh, int kw, cudaStream_t s, int *rc);  // box_stream.cu
+
+// The focal statistics of one raster: stat is one xrs_focal_stat, written to planes.p[stat], or kAllStats for
+// every plane that is set.  A wide window takes the ring kernel; a single mean over an all-ones window the running
+// box; a raster TMA can describe the tiled kernel, one launch for all the planes; any other raster the
+// bounds-checked kernel, one plane at a time.
+static int focal_stats(const float *in, int64_t in_pitch, const StatPlanes &planes, int64_t out_pitch, int64_t H,
+                       int64_t W, const double *kernel, int kh, int kw, int stat, cudaStream_t s) {
+    if (is_wide(kh, kw)) return focal_wide(in, in_pitch, planes, out_pitch, H, W, kernel, kh, kw, stat, s);
+    static thread_local MaskBits mask;
+    const bool all_ones = mask_bits(mask, kernel, kh, kw);
+    if (stat == XRS_STAT_MEAN && all_ones) {  // np.ones((k, k)): the running box, O(1) per cell
+        int brc = XRS_OK;
+        if (try_box_nanmean(in, in_pitch, planes.p[stat], out_pitch, H, W, kh, kw, s, &brc)) return brc;
+    }
+    float *out = nullptr;  // any plane: the planes share their alignment
+    for (float *p : planes.p)
+        if (p) out = p;
+    TileGeom g;
+    CUtensorMap tmap;
+    if (tile_geom(g, &tmap, in, in_pitch, out, out_pitch, H, W, kh, kw, kTileH))
+        return with_stat(stat, [&](auto S) {
+            // at most 3 CTAs per SM (registers differ a lot between the statistics): the tile loop is persistent
+            return launch_tiles(focal_tile_kernel<S>, g, 3, s, S == kAllStats ? kFocalFused : kFocalTiled, tmap,
+                                mask, focal_out<S>(planes), out_pitch / 4, g);
+        });
+    const int64_t cell_ctas = (H * W + 255) / 256, max_ctas = (int64_t)sm_count() * 8;
+    for (int i = 0; i < 7; ++i) {
+        if (!planes.p[i]) continue;
+        const int rc = launch(focal_stat_direct_kernel, cell_ctas < max_ctas ? cell_ctas : max_ctas, 256, 0, s,
+                              kFocalDirect, in, in_pitch / 4, mask, planes.p[i], out_pitch / 4, H, W, kh, kw, i);
+        if (rc) return rc;
+    }
+    return XRS_OK;
+}
 }
 
 extern "C" {
@@ -1076,39 +999,9 @@ int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
     const int rc = check_common(in, in_pitch, out, out_pitch, H, W, kernel, kh, kw);
     if (rc) return rc;
     XRS_REQUIRE(stat >= XRS_STAT_MEAN && stat <= XRS_STAT_VAR, "unknown focal statistic");
-    if (is_wide(kh, kw)) {
-        StatPlanes planes = {};
-        planes.p[stat] = out;
-        return focal_wide(in, in_pitch, planes, out_pitch, H, W, kernel, kh, kw, stat, (cudaStream_t)s);
-    }
-    static thread_local MaskBits mask;
-    bool all_ones = true;
-    for (int i = 0; i < kh * kw; ++i) {
-        mask.m[i] = (kernel[i] == 1.0) ? 1 : 0;  // focal.py:323
-        all_ones = all_ones && mask.m[i];
-    }
-    if (stat == XRS_STAT_MEAN && all_ones) {   // np.ones((k, k)): the running box, O(1) per cell
-        int brc = XRS_OK;
-        if (try_box_nanmean(in, in_pitch, out, out_pitch, H, W, kh, kw, (cudaStream_t)s, &brc)) return brc;
-    }
-    TileGeom g;
-    CUtensorMap tmap;
-    if (tile_geom(g, &tmap, in, in_pitch, out, out_pitch, H, W, kh, kw, kTileH)) {
-        auto kern = focal_stat_kernel<XRS_STAT_MEAN>;
-        switch (stat) {
-            case XRS_STAT_SUM: kern = focal_stat_kernel<XRS_STAT_SUM>; break;
-            case XRS_STAT_MIN: kern = focal_stat_kernel<XRS_STAT_MIN>; break;
-            case XRS_STAT_MAX: kern = focal_stat_kernel<XRS_STAT_MAX>; break;
-            case XRS_STAT_STD: kern = focal_stat_kernel<XRS_STAT_STD>; break;
-            case XRS_STAT_RANGE: kern = focal_stat_kernel<XRS_STAT_RANGE>; break;
-            case XRS_STAT_VAR: kern = focal_stat_kernel<XRS_STAT_VAR>; break;
-        }
-        // at most 3 CTAs per SM (registers differ a lot between the statistics): the tile loop is persistent
-        return launch_tiles(kern, g, 3, (cudaStream_t)s, kFocalTiled, tmap, mask, out, out_pitch / 4, g);
-    }
-    const int64_t cell_ctas = (H * W + 255) / 256, max_ctas = (int64_t)sm_count() * 8;
-    return launch(focal_stat_direct_kernel, cell_ctas < max_ctas ? cell_ctas : max_ctas, 256, 0, (cudaStream_t)s,
-                  kFocalDirect, in, in_pitch / 4, mask, out, out_pitch / 4, H, W, kh, kw, stat);
+    StatPlanes planes = {};
+    planes.p[stat] = out;
+    return focal_stats(in, in_pitch, planes, out_pitch, H, W, kernel, kh, kw, stat, (cudaStream_t)s);
 }
 
 int xrs_focal_stats_multi_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t plane_stride,
@@ -1119,29 +1012,15 @@ int xrs_focal_stats_multi_f32(const float *in, int64_t in_pitch, float *out, int
     if (H <= 0 || W <= 0) return XRS_OK;
     const int rc = check_common(in, in_pitch, out, out_pitch, H, W, kernel, kh, kw);
     if (rc) return rc;
-    StatPlanes planes;
-    for (auto &p : planes.p) p = nullptr;
+    StatPlanes planes = {};
     for (int i = 0; i < n_stats; ++i) {
         XRS_REQUIRE(stats[i] >= XRS_STAT_MEAN && stats[i] <= XRS_STAT_VAR, "unknown focal statistic");
         XRS_REQUIRE(planes.p[stats[i]] == nullptr, "statistic requested twice");
         planes.p[stats[i]] = reinterpret_cast<float *>(reinterpret_cast<char *>(out) + (int64_t)i * plane_stride);
     }
-    if (is_wide(kh, kw))
-        return focal_wide(in, in_pitch, planes, out_pitch, H, W, kernel, kh, kw, kAllStats, (cudaStream_t)s);
-    TileGeom g;
-    CUtensorMap tmap;
-    if (n_stats >= 2 && tile_geom(g, &tmap, in, in_pitch, out, out_pitch, H, W, kh, kw, kTileH)) {
-        static thread_local MaskBits mask;
-        for (int i = 0; i < kh * kw; ++i) mask.m[i] = (kernel[i] == 1.0) ? 1 : 0;  // focal.py:323
-        return launch_tiles(focal_stats_multi_kernel, g, 3, (cudaStream_t)s, kFocalFused, tmap, mask, planes,
-                            out_pitch / 4, g);
-    }
-    // single statistic, or a raster TMA cannot describe: one launch per plane
-    for (int i = 0; i < n_stats; ++i) {
-        const int r2 = xrs_focal_stat_f32(in, in_pitch, planes.p[stats[i]], out_pitch, H, W, kernel, kh, kw, stats[i], s);
-        if (r2) return r2;
-    }
-    return XRS_OK;
+    // one statistic takes its own kernels
+    return focal_stats(in, in_pitch, planes, out_pitch, H, W, kernel, kh, kw, n_stats == 1 ? stats[0] : kAllStats,
+                       (cudaStream_t)s);
 }
 
 }  // extern "C"

@@ -143,7 +143,9 @@ def _focal_stats_cupy(data, kernel, stats_funcs):
     H, W = t.shape
     k = np.ascontiguousarray(kernel, dtype=np.float64)
     ids = (ctypes.c_int * len(stats_funcs))(*[_lib.STATS[s] for s in stats_funcs])
-    out = torch.empty((len(stats_funcs), H, W), dtype=torch.float32, device=t.device)
+    plane = (H * W + 3) // 4 * 4          # planes start on 16-byte boundaries
+    out = torch.empty(len(stats_funcs) * plane, dtype=torch.float32, device=t.device)
+    out = out.as_strided((len(stats_funcs), H, W), (plane, W, 1))
     if H and W:
         with torch.cuda.device(t.device):
             _lib.call("xrs_focal_stats_multi_f32", ctypes.c_void_p(t.data_ptr()), t.stride(0) * 4,
@@ -165,9 +167,8 @@ def focal_stats(agg, kernel, stats_funcs=['mean', 'max', 'min', 'range', 'std', 
             raise ValueError("unknown focal statistic %r" % (stats,))
     stats_funcs = list(stats_funcs)
     index = pd.Index(stats_funcs, name='stats', dtype=object)
-    if is_device_array(agg.data) and len(set(stats_funcs)) == len(stats_funcs) and 2 <= len(stats_funcs) <= 7 \
-            and agg.shape[1] % 4 == 0:
-        # one fused pass writing straight into the stacked result
+    if stats_funcs and is_device_array(agg.data) and len(set(stats_funcs)) == len(stats_funcs):
+        # one call writing straight into the stacked result (the C entry point rejects a repeated statistic)
         data = _focal_stats_cupy(agg.data, kernel, stats_funcs)
         coords = OrderedDict()
         coords['stats'] = np.asarray(stats_funcs, dtype=object)
