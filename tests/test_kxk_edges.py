@@ -317,7 +317,7 @@ def test_ragged_width_falls_back_per_plane(lib):
 
 # ------------------------------------------------------------------------------------------------ running box
 def _box_rows(lib, H, W, kh, kw):
-    """Rows where the launcher's row segments start (2 CTAs per SM, as launch_box_stream2 asks for), the
+    """Rows where the launcher's row segments start (2 CTAs per SM, as launch_box_stream asks for), the
     raster's first and last kh rows, and the rows at both sides of a 4-row batch."""
     l = lib.lib()
     n = ctypes.c_int(0)

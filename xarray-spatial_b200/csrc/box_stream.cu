@@ -1,6 +1,7 @@
 // box_stream.cu -- convolve_2d with a kernel whose taps are all the same weight w
 // (np.ones((k, k)) / k**2: the mean filter of the reference's docs and of benchmarks/; also any
-// rectangular kh x kw): out = w * (sum of the window), reference convolution.py:285-313.
+// rectangular kh x kw): out = w * (sum of the window), reference convolution.py:285-313.  The same kernel body
+// serves focal.apply's mean over an all-ones window (BoxNanMean below, focal.py:305-326).
 //
 // A separable RUNNING box on a CTA-wide TMA pipeline: O(1) work per cell for every k.
 //   * vertical: every lane keeps the running column sums V of its 4 columns over the last kh rows in
@@ -48,8 +49,7 @@ constexpr int kBsWarps = 7;      // consumer warps per CTA (+ 1 producer warp)
 constexpr int kBsMaxK = 25;      // window rows / columns served
 constexpr float kBsHuge = 1.2676506e30f;  // 2^100: the cut-off when the sample holds no finite nonzero cell
 constexpr float kBsScale = 32768.f;       // 2^15: cells at or above kBsScale x the sample median are exceptional
-constexpr int kB2Rows = 4;       // rows per stage half (entering / leaving)
-constexpr int kBoxNotTaken = -12345;
+constexpr int kBoxRows = 4;      // rows per stage half (entering / leaving)
 
 // The launch's cut-off between ordinary cells (summed into V) and exceptional ones (kept out of V, their windows
 // recomputed tap by tap): 2^15 x the median |x| of the finite nonzero cells among 128 fixed sample cells
@@ -124,25 +124,25 @@ __device__ __forceinline__ double bs_div_n(double c, double n, double inv) {
     return fma(fma(-q, n, c), inv, q);
 }
 
-template <int RX, int NW> struct B2Shape {
+template <int RX, int NW> struct BoxShape {
     static constexpr int kPad = (RX + 3) / 4 * 4;               // columns a warp cannot emit on each side
     static constexpr int kOutW = kStripW - 2 * kPad;            // columns a warp emits
     static constexpr int kTileOutW = NW * kOutW;
     static constexpr int kTileInW = kTileOutW + 2 * kPad;
     static constexpr int kNBox = (kTileInW + 255) / 256;
     static constexpr int kBoxW = ((kTileInW + kNBox - 1) / kNBox + 31) / 32 * 32;   // cells: 128-byte multiples
-    static constexpr int kBoxCells = kB2Rows * kBoxW;           // one TMA box: 4 rows x kBoxW cells
+    static constexpr int kBoxCells = kBoxRows * kBoxW;          // one TMA box: 4 rows x kBoxW cells
     static constexpr int kHalfCells = kNBox * kBoxCells;        // the entering (or leaving) rows of a stage
     static constexpr uint32_t kHalfBytes = kHalfCells * 4;
     static_assert(kBoxW <= 256 && kBoxW % 32 == 0 && kNBox * kBoxW >= kTileInW, "TMA box geometry");
 };
 
-struct B2Geom {
+struct BoxGeom {
     int64_t H, W;
     int kh, ry;
     int n_tiles, n_segs, seg_rows;
     int stages;
-    double w;        // MODE 0: the taps' common weight; MODE 1: 1 / (kh * kw)
+    double w;        // convolve: the taps' common weight; mean: 1 / (kh * kw)
     double n_cells;  // kh * kw
 };
 
@@ -230,14 +230,107 @@ __device__ __forceinline__ void bs_lanesum(const T (&v)[R][4], T (&win)[R][4]) {
 
 __device__ __forceinline__ uint32_t bs_bits(int n) { return n >= 32 ? 0xffffffffu : ((1u << n) - 1u); }
 
-// MODE 0: convolve_2d (a NaN anywhere in the window makes the result NaN; raster-edge windows are NaN).
-// MODE 1: focal.apply mean over an all-ones window (NaN and out-of-raster cells are skipped).
-template <int RX, int NW, int MODE>
+// The kernel's two modes: which loaded cells read as 0, how a window sum becomes the float32 output and how a window
+// holding NaN / inf / huge cells is finished.  Built per task for the lane whose first cell is raster column x.
+
+// convolve_2d: out = w * (sum of the window).  A NaN anywhere in the window makes the result NaN, so the columns
+// beyond the raster's left / right edge (NaN from the TMA unit) need no masking: they poison exactly their own lane's
+// sums, and the windows that contain them come out NaN like the reference's.
+template <int RX> struct BoxConvolve {
+    __device__ __forceinline__ BoxConvolve(const BoxGeom &, int64_t, bool) {}
+    // whether the lane's cells read as 0 in the fast path (FAST) or in the row-by-row path
+    template <bool FAST> __device__ __forceinline__ bool zeroes() const { return false; }
+    static constexpr bool edge_warp = false;
+    // the output of column j's window sum; EDGE: in a warp at the raster's left / right edge
+    template <bool EDGE> __device__ __forceinline__ float out(const BoxGeom &g, double win, int) const {
+        return (float)fma(g.w, win, 0.0);   // + 0.0: an all-zero window is +0 like the reference's
+    }
+    // res of column j, whose window holds NaN cells (the low 16 bits of n) or infinite / huge ones (the high 16 bits);
+    // `direct`: the lane stores, so the window may be recomputed from `in`
+    __device__ __forceinline__ void finish_exceptional(float &res, int j, double win, unsigned n, bool direct,
+                                                       const float *in, int64_t pitch, const BoxGeom &g, int64_t y,
+                                                       int64_t x) const {
+        if (n & 0xffffu) res = nan_of<float>();
+        else if ((n >> 16) && direct) res = bs_direct(in, pitch, g.H, g.W, y, x + j, g.kh, 2 * RX + 1, g.w);
+    }
+};
+
+// focal.apply's mean over an all-ones window: NaN cells and cells beyond the raster are skipped.  Out-of-raster lanes
+// read as 0, and a window that reaches over the raster's left / right edge divides by kh x the columns it really has
+// (ncv): edge tiles stay on the fast path.
+template <int RX> struct BoxNanMean {
+    int ncv[4];       // raster columns in the windows of the lane's 4 columns
+    bool edge_warp;   // warp-uniform: a window of the warp reaches beyond the raster's left / right edge
+    bool outside;     // the lane's cells lie beyond the raster
+    __device__ __forceinline__ BoxNanMean(const BoxGeom &g, int64_t x, bool in_raster) : outside(!in_raster) {
+        bool edge_lane = false;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int64_t xc = x + j;
+            const int64_t lo = xc - RX < 0 ? 0 : xc - RX, hi = xc + RX > g.W - 1 ? g.W - 1 : xc + RX;
+            ncv[j] = (int)(hi - lo + 1);
+            edge_lane = edge_lane || (ncv[j] != 2 * RX + 1);
+        }
+        edge_warp = __any_sync(0xffffffffu, edge_lane && in_raster);
+    }
+    // the fast path tests only the warps at the raster's edges, the only ones whose outputs read such lanes (a warp-
+    // uniform branch); the row-by-row path zeroes every out-of-raster lane
+    template <bool FAST> __device__ __forceinline__ bool zeroes() const { return FAST ? edge_warp && outside : outside; }
+    template <bool EDGE> __device__ __forceinline__ float out(const BoxGeom &g, double win, int j) const {
+        return EDGE ? (float)(win / (double)(g.kh * ncv[j])) : (float)bs_div_n(win, g.n_cells, g.w);
+    }
+    __device__ __forceinline__ void finish_exceptional(float &res, int j, double win, unsigned n, bool direct,
+                                                       const float *in, int64_t pitch, const BoxGeom &g, int64_t y,
+                                                       int64_t x) const {
+        if (n >> 16) {   // infinite / huge cells take part: the reference's order
+            if (direct) res = bs_direct_nanmean(in, pitch, g.H, g.W, y, x + j, g.kh, 2 * RX + 1);
+        } else if (n & 0xffffu) {
+            res = (float)(win / (double)(g.kh * ncv[j] - (int)(n & 0xffffu)));   // all skipped: 0 / 0 = NaN
+        }
+    }
+};
+
+// the lane's 4 cells of one stage row, in the fast path (FAST) or the row-by-row path; the lanes the mode zeroes read 0
+template <bool FAST, typename M> __device__ __forceinline__ void bs_row(const M &m, const float *p, float (&v)[4]) {
+    const float4 q = *reinterpret_cast<const float4 *>(p);
+    v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+    if (m.template zeroes<FAST>()) { v[0] = 0.f; v[1] = 0.f; v[2] = 0.f; v[3] = 0.f; }
+}
+
+// the lane's 4 outputs of one row
+template <bool EDGE, typename M>
+__device__ __forceinline__ void bs_store(const M &m, float *p, const BoxGeom &g, const double (&win)[4]) {
+    __stcs(reinterpret_cast<float4 *>(p), make_float4(m.template out<EDGE>(g, win[0], 0), m.template out<EDGE>(g, win[1], 1),
+                                                      m.template out<EDGE>(g, win[2], 2), m.template out<EDGE>(g, win[3], 3)));
+}
+
+// adds (SIGN = 1) or retires (SIGN = -1) a row of the window in the column sums V.  In a dirty row (one the warp
+// voted to hold a NaN / inf / huge cell) such cells stay out of V and are counted in C instead.
+template <int SIGN>
+__device__ __forceinline__ void bs_update(double (&V)[4], unsigned (&C)[4], const float (&v)[4], bool dirty, float thr) {
+    if (!dirty) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if constexpr (SIGN > 0) V[j] += (double)v[j]; else V[j] -= (double)v[j];
+        }
+    } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const bool isnan_ = v[j] != v[j];
+            const bool big = !isnan_ && !(fabsf(v[j]) < thr);
+            const double d = (isnan_ || big) ? 0.0 : (double)v[j];
+            const unsigned c = isnan_ ? 1u : (big ? 0x10000u : 0u);
+            if constexpr (SIGN > 0) { V[j] += d; C[j] += c; } else { V[j] -= d; C[j] -= c; }
+        }
+    }
+}
+
+// M: BoxConvolve or BoxNanMean
+template <int RX, int NW, template <int> class M>
 __global__ void __launch_bounds__((NW + 1) * 32, 2)
-box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__restrict__ in, int64_t in_pitch_elems,
-                   float *__restrict__ out, int64_t out_pitch_elems, const B2Geom g) {
-    using S = B2Shape<RX, NW>;
-    constexpr int kw = 2 * RX + 1;
+box_stream_kernel(const __grid_constant__ CUtensorMap tmap, const float *__restrict__ in, int64_t in_pitch_elems,
+                  float *__restrict__ out, int64_t out_pitch_elems, const BoxGeom g) {
+    using S = BoxShape<RX, NW>;
     constexpr int kStageCells = 2 * S::kHalfCells;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     float *ring = reinterpret_cast<float *>(smem_raw);
@@ -269,9 +362,9 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
                 const int bx = tile * S::kTileOutW - S::kPad;
                 const int ytop = (int)y0 - ry;
                 const int n_in = (int)(y1 - y0) + kh - 1;
-                for (int e0 = 0; e0 < n_in; e0 += kB2Rows) {
+                for (int e0 = 0; e0 < n_in; e0 += kBoxRows) {
                     mbar_wait(&empty[stage], lap ^ 1u);  // a fresh barrier passes the first lap
-                    const bool leaving = e0 + kB2Rows - 1 >= kh - 1;
+                    const bool leaving = e0 + kBoxRows - 1 >= kh - 1;
                     mbar_arrive_expect_tx(&full[stage], leaving ? 2u * S::kHalfBytes : S::kHalfBytes);
                     float *dst = ring + (size_t)stage * kStageCells;
 #pragma unroll
@@ -303,126 +396,69 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
         const int64_t y0 = (int64_t)seg * g.seg_rows, y1 = min(y0 + (int64_t)g.seg_rows, g.H);
         const int64_t x = (int64_t)tile * S::kTileOutW - S::kPad + col;  // raster column of the lane's first cell
         const bool in_raster = x >= 0 && x < g.W;                          // W % 4 == 0: all four cells in or out
-        const bool store_ok = emits && in_raster;
-        // Out-of-raster columns (NaN from the TMA unit) never vote a row "dirty".  MODE 0: they may poison
-        // their own lane's sums -- exactly the windows that contain them must be NaN.  MODE 1 skips them: the
-        // lane's cells are read as 0, and a window that reaches beyond the raster's left / right edge divides
-        // by the number of columns it really has (ncv) -- edge tiles stay on the fast path in both modes.
-        const bool watch = in_raster;
-        int ncv[4] = {kw, kw, kw, kw};
-        bool edge_warp = false;
-        if constexpr (MODE == 1) {
-            bool edge_lane = false;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int64_t xc = x + j;
-                const int64_t lo = xc - RX < 0 ? 0 : xc - RX, hi = xc + RX > g.W - 1 ? g.W - 1 : xc + RX;
-                ncv[j] = (int)(hi - lo + 1);
-                edge_lane = edge_lane || (ncv[j] != kw);
-            }
-            edge_warp = __any_sync(0xffffffffu, edge_lane && in_raster);
-        }
+        const bool store_ok = emits && in_raster;                           // out-of-raster lanes never vote a row dirty
+        const M<RX> m(g, x, in_raster);
         float *optr = out + y0 * out_pitch_elems + x;
 
         double V[4] = {0.0, 0.0, 0.0, 0.0};
         unsigned C[4] = {0u, 0u, 0u, 0u};   // lo 16 bits: NaN cells in the column window, hi 16: infinite / huge
         uint32_t dirty = 0;                  // bit i: the row added i rows ago held a NaN / inf / huge cell (this warp)
         const int n_in = (int)(y1 - y0) + kh - 1;
-        for (int e0 = 0; e0 < n_in; e0 += kB2Rows) {
+        for (int e0 = 0; e0 < n_in; e0 += kBoxRows) {
             mbar_wait(&full[stage], lap);
             const float *se = ring + (size_t)stage * kStageCells + off;   // entering rows
             const float *sl = se + S::kHalfCells;                          // leaving rows
             bool done = false;
-            if (e0 >= kh - 1 && e0 + kB2Rows <= n_in && (dirty & win_mask) == 0u) {
+            if (e0 >= kh - 1 && e0 + kBoxRows <= n_in && (dirty & win_mask) == 0u) {
                 // ---- fast path: window complete, 4 rows enter, 4 rows are emitted, 4 rows leave; neither
                 // the window nor the entering rows hold a NaN / inf / huge cell inside the raster
-                float nv[kB2Rows][4];
+                float nv[kBoxRows][4];
 #pragma unroll
-                for (int i = 0; i < kB2Rows; ++i) {
-                    const float4 q = *reinterpret_cast<const float4 *>(se + i * S::kBoxW);
-                    nv[i][0] = q.x; nv[i][1] = q.y; nv[i][2] = q.z; nv[i][3] = q.w;
-                }
-                if constexpr (MODE == 1) {
-                    if (edge_warp && !in_raster) {   // only warps at the raster's left / right edge hold such lanes
-#pragma unroll
-                        for (int i = 0; i < kB2Rows; ++i) { nv[i][0] = 0.f; nv[i][1] = 0.f; nv[i][2] = 0.f; nv[i][3] = 0.f; }
-                    }
-                }
+                for (int i = 0; i < kBoxRows; ++i) bs_row<true>(m, se + i * S::kBoxW, nv[i]);
                 const float amax = bs_amax3(bs_amax3(bs_amax4(nv[0]), nv[1][0], nv[1][1]),
                                             bs_amax3(bs_amax4(nv[2]), nv[1][2], nv[1][3]), bs_amax4(nv[3]));
-                if (!__any_sync(0xffffffffu, watch && !(amax < thr))) {
-                    float ov[kB2Rows][4];
+                if (!__any_sync(0xffffffffu, in_raster && !(amax < thr))) {
+                    float ov[kBoxRows][4];
 #pragma unroll
-                    for (int i = 0; i < kB2Rows; ++i) {
-                        const float4 q = *reinterpret_cast<const float4 *>(sl + i * S::kBoxW);
-                        ov[i][0] = q.x; ov[i][1] = q.y; ov[i][2] = q.z; ov[i][3] = q.w;
-                    }
-                    if constexpr (MODE == 1) {
-                        if (edge_warp && !in_raster) {
-#pragma unroll
-                            for (int i = 0; i < kB2Rows; ++i) { ov[i][0] = 0.f; ov[i][1] = 0.f; ov[i][2] = 0.f; ov[i][3] = 0.f; }
-                        }
-                    }
+                    for (int i = 0; i < kBoxRows; ++i) bs_row<true>(m, sl + i * S::kBoxW, ov[i]);
                     // column sums of output row i: V_i = V_{i-1} - old_{i-1} + new_i
-                    double P[kB2Rows][4];
+                    double P[kBoxRows][4];
 #pragma unroll
                     for (int j = 0; j < 4; ++j) {
                         double acc = V[j];
 #pragma unroll
-                        for (int i = 0; i < kB2Rows; ++i) {
+                        for (int i = 0; i < kBoxRows; ++i) {
                             const double d = (i == 0) ? (double)nv[0][j] : ((double)nv[i][j] - (double)ov[i > 0 ? i - 1 : 0][j]);
                             acc += d;
                             P[i][j] = acc;
                         }
-                        V[j] = acc - (double)ov[kB2Rows - 1][j];
+                        V[j] = acc - (double)ov[kBoxRows - 1][j];
                     }
-                    double win[kB2Rows][4];
-                    bs_lanesum<RX, kB2Rows, double>(P, win);
+                    double win[kBoxRows][4];
+                    bs_lanesum<RX, kBoxRows, double>(P, win);
 #pragma unroll
-                    for (int i = 0; i < kB2Rows; ++i) {
+                    for (int i = 0; i < kBoxRows; ++i) {
                         if (store_ok) {
-                            if constexpr (MODE == 0)
-                                __stcs(reinterpret_cast<float4 *>(optr),
-                                       make_float4((float)fma(g.w, win[i][0], 0.0), (float)fma(g.w, win[i][1], 0.0),
-                                                   (float)fma(g.w, win[i][2], 0.0), (float)fma(g.w, win[i][3], 0.0)));
-                            else if (!edge_warp)
-                                __stcs(reinterpret_cast<float4 *>(optr),
-                                       make_float4((float)bs_div_n(win[i][0], g.n_cells, g.w), (float)bs_div_n(win[i][1], g.n_cells, g.w),
-                                                   (float)bs_div_n(win[i][2], g.n_cells, g.w), (float)bs_div_n(win[i][3], g.n_cells, g.w)));
-                            else
-                                __stcs(reinterpret_cast<float4 *>(optr),
-                                       make_float4((float)(win[i][0] / (double)(kh * ncv[0])), (float)(win[i][1] / (double)(kh * ncv[1])),
-                                                   (float)(win[i][2] / (double)(kh * ncv[2])), (float)(win[i][3] / (double)(kh * ncv[3]))));
+                            if (!m.edge_warp) bs_store<false>(m, optr, g, win[i]);   // warp-uniform
+                            else bs_store<true>(m, optr, g, win[i]);
                         }
                         optr += out_pitch_elems;
                     }
-                    dirty <<= kB2Rows;
+                    dirty <<= kBoxRows;
                     done = true;
                 }
             }
             if (!done) {
                 // ---- row by row: lead-in rows (nothing to emit yet), the last rows of a task, and windows
                 // or entering rows with NaN / inf / huge cells (kept out of V, counted in C)
-                for (int i = 0; i < kB2Rows; ++i) {
+                for (int i = 0; i < kBoxRows; ++i) {
                     const int e = e0 + i;
                     if (e >= n_in) break;
-                    const float4 q = *reinterpret_cast<const float4 *>(se + i * S::kBoxW);
-                    const bool zero_lane = MODE == 1 && !in_raster;
-                    const float v[4] = {zero_lane ? 0.f : q.x, zero_lane ? 0.f : q.y, zero_lane ? 0.f : q.z, zero_lane ? 0.f : q.w};
-                    const bool row_dirty = __any_sync(0xffffffffu, watch && !(bs_amax4(v) < thr));
+                    float v[4];
+                    bs_row<false>(m, se + i * S::kBoxW, v);
+                    const bool row_dirty = __any_sync(0xffffffffu, in_raster && !(bs_amax4(v) < thr));
                     dirty = (dirty << 1) | (row_dirty ? 1u : 0u);
-                    if (!row_dirty) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) V[j] += (double)v[j];
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const bool isnan_ = v[j] != v[j];
-                            const bool big = !isnan_ && !(fabsf(v[j]) < thr);
-                            V[j] += (isnan_ || big) ? 0.0 : (double)v[j];
-                            C[j] += isnan_ ? 1u : (big ? 0x10000u : 0u);
-                        }
-                    }
+                    bs_update<1>(V, C, v, row_dirty, thr);
                     if (e < kh - 1) continue;   // window not complete yet
 
                     // emit output row y = y0 + e - (kh - 1)
@@ -432,47 +468,22 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
                     float res[4];
 #pragma unroll
                     for (int j = 0; j < 4; ++j)
-                        res[j] = MODE == 0 ? (float)fma(g.w, w1[0][j], 0.0)    // + 0.0: an all-zero window is +0 like the reference's
-                                 : (edge_warp ? (float)(w1[0][j] / (double)(kh * ncv[j])) : (float)bs_div_n(w1[0][j], g.n_cells, g.w));
+                        res[j] = m.edge_warp ? m.template out<true>(g, w1[0][j], j) : m.template out<false>(g, w1[0][j], j);
                     if (win_dirty) {   // warp-uniform
                         unsigned C1[1][4] = {{C[0], C[1], C[2], C[3]}}, wc[1][4];
                         bs_lanesum<RX, 1, unsigned>(C1, wc);
                         const int64_t y = y0 + e - (kh - 1);
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            if constexpr (MODE == 0) {
-                                if (wc[0][j] & 0xffffu) res[j] = nan_of<float>();
-                                else if (wc[0][j] >> 16) {
-                                    if (store_ok) res[j] = bs_direct(in, in_pitch_elems, g.H, g.W, y, x + j, kh, kw, g.w);
-                                }
-                            } else {
-                                if (wc[0][j] >> 16) {          // infinite / huge cells take part: the reference's order
-                                    if (store_ok) res[j] = bs_direct_nanmean(in, in_pitch_elems, g.H, g.W, y, x + j, kh, kw);
-                                } else if (wc[0][j] & 0xffffu) {
-                                    res[j] = (float)(w1[0][j] / (double)(kh * ncv[j] - (int)(wc[0][j] & 0xffffu)));   // all skipped: 0 / 0 = NaN
-                                }
-                            }
-                        }
+                        for (int j = 0; j < 4; ++j)
+                            m.finish_exceptional(res[j], j, w1[0][j], wc[0][j], store_ok, in, in_pitch_elems, g, y, x);
                     }
                     if (store_ok) __stcs(reinterpret_cast<float4 *>(optr), make_float4(res[0], res[1], res[2], res[3]));
                     optr += out_pitch_elems;
 
                     // retire input row e - (kh - 1), the oldest row of the window
-                    const float4 qo = *reinterpret_cast<const float4 *>(sl + i * S::kBoxW);
-                    const float vo[4] = {zero_lane ? 0.f : qo.x, zero_lane ? 0.f : qo.y, zero_lane ? 0.f : qo.z, zero_lane ? 0.f : qo.w};
-                    const bool old_dirty = (dirty >> (kh - 1)) & 1u;
-                    if (!old_dirty) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) V[j] -= (double)vo[j];
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const bool isnan_ = vo[j] != vo[j];
-                            const bool big = !isnan_ && !(fabsf(vo[j]) < thr);
-                            V[j] -= (isnan_ || big) ? 0.0 : (double)vo[j];
-                            C[j] -= isnan_ ? 1u : (big ? 0x10000u : 0u);
-                        }
-                    }
+                    float vo[4];
+                    bs_row<false>(m, sl + i * S::kBoxW, vo);
+                    bs_update<-1>(V, C, vo, (dirty >> (kh - 1)) & 1u, thr);
                 }
             }
             __syncwarp();
@@ -482,79 +493,55 @@ box_stream2_kernel(const __grid_constant__ CUtensorMap tmap, const float *__rest
     }
 }
 
-template <int RX, int NW, int MODE>
-static int launch_box_stream2(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
-                              int kh, double w, cudaStream_t s) {
-    using S = B2Shape<RX, NW>;
-    CUtensorMap tmap;
-    if (!make_tensor_map_2d(&tmap, in, in_pitch, H, W, XRS_F32, S::kBoxW, kB2Rows)) return kBoxNotTaken;
-    B2Geom g;
+template <int RX, template <int> class M>
+static int launch_box_stream(const CUtensorMap &tmap, const float *in, int64_t in_pitch, float *out, int64_t out_pitch,
+                             int64_t H, int64_t W, int kh, double w, cudaStream_t s) {
+    using S = BoxShape<RX, kBsWarps>;
+    BoxGeom g;
     g.H = H; g.W = W; g.kh = kh; g.ry = kh / 2; g.w = w;
     g.n_cells = (double)(kh * (2 * RX + 1));
     g.n_tiles = (int)((W + S::kTileOutW - 1) / S::kTileOutW);
-    int stages = RX <= 2 ? 3 : 4, max_ctas = 2, want = 4;   // swept with scripts/tune/box_zonal_sweep.py
-    if (const char *e = getenv("XRS_BOX_STAGES")) stages = atoi(e);
-    if (const char *e = getenv("XRS_BOX_CTAS")) max_ctas = atoi(e);
-    if (const char *e = getenv("XRS_BOX_WAVES")) want = atoi(e);
-    if (max_ctas < 1) max_ctas = 1;
-    if (want < 1) want = 1;
-    const size_t stage_bytes = (size_t)2 * S::kHalfBytes;
-    const size_t cap = (kSmemPerSm - (size_t)max_ctas * kSmemReservedPerCta) / max_ctas - 256;
-    if (stages < 2) stages = 2;
-    while (stages > 2 && (size_t)stages * stage_bytes + (size_t)2 * stages * sizeof(uint64_t) > cap) --stages;
-    g.stages = stages;
-    const size_t smem = (size_t)stages * stage_bytes + (size_t)2 * stages * sizeof(uint64_t);
-    auto kern = box_stream2_kernel<RX, NW, MODE>;
+    // 3 stages up to radius 2 and 4 above, at most 2 CTAs per SM, row segments for 4 waves of tasks: the fastest
+    // setting of a sweep of 2 .. 6 stages, 1 / 2 CTAs per SM and 2 .. 8 waves at k = 5, 9, 15, 25 over a 32768^2
+    // DEM, run on a B200 when the kernel was written and not repeated on the H100
+    g.stages = RX <= 2 ? 3 : 4;
+    const size_t smem = (size_t)g.stages * (2 * S::kHalfBytes + 2 * sizeof(uint64_t));
+    static_assert(4 * (2 * S::kHalfBytes + 2 * sizeof(uint64_t)) <= (kSmemPerSm - 2 * kSmemReservedPerCta) / 2 - 256,
+                  "4 stages for each of 2 CTAs per SM");
+    auto kern = box_stream_kernel<RX, kBsWarps, M>;
     int64_t resident;
-    if (const int rc = resident_ctas(kern, (NW + 1) * 32, smem, max_ctas, &resident)) return rc;
+    if (const int rc = resident_ctas(kern, (kBsWarps + 1) * 32, smem, 2, &resident)) return rc;
     // segments: tall enough that the kh - 1 lead-in rows stay a small overhead, (rows + kh - 1) a
     // multiple of 4 so that only the raster's last segment ends in a partial batch
-    const int64_t seg_rows = pick_seg_rows(H, g.n_tiles, resident, 12 * (int64_t)kh, kh - 1, kB2Rows, want);
+    const int64_t seg_rows = pick_seg_rows(H, g.n_tiles, resident, 12 * (int64_t)kh, kh - 1, kBoxRows, 4);
     g.seg_rows = (int)seg_rows;
     g.n_segs = (int)((H + seg_rows - 1) / seg_rows);
     const int64_t n_tasks = (int64_t)g.n_tiles * g.n_segs;
-    return launch(kern, resident < n_tasks ? resident : n_tasks, (NW + 1) * 32, smem, s, kRunningBox, tmap, in,
+    return launch(kern, resident < n_tasks ? resident : n_tasks, (kBsWarps + 1) * 32, smem, s, kRunningBox, tmap, in,
                   in_pitch / 4, out, out_pitch / 4, g);
 }
 
-// true when the streaming box kernel took the job (*rc = its status)
-bool try_box_stream(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
-                    const double *kernel, int kh, int kw, cudaStream_t s, int *rc) {
-    if (kh > kBsMaxK || kw > kBsMaxK || kh < 1 || kw < 3 || (kw & 1) == 0 || (kh & 1) == 0) return false;
-    const double w = kernel[0];
-    if (!(fabs(w) <= 1.7976931348623157e308)) return false;
-    for (int i = 1; i < kh * kw; ++i)
-        if (memcmp(&kernel[i], &w, sizeof(double)) != 0) return false;
-    if (W % 4 != 0 || out_pitch % 16 != 0 || (reinterpret_cast<uintptr_t>(out) & 15)) return false;
-    if (H >= (1LL << 31) - 64 || W >= (1LL << 31) - 4096) return false;
-    int r2 = kBoxNotTaken;
-    switch (kw / 2) {
-#define XRS_BS(R) case R: r2 = launch_box_stream2<R, kBsWarps, 0>(in, in_pitch, out, out_pitch, H, W, kh, w, s); break;
-        XRS_BS(1) XRS_BS(2) XRS_BS(3) XRS_BS(4) XRS_BS(5) XRS_BS(6) XRS_BS(7) XRS_BS(8) XRS_BS(9) XRS_BS(10) XRS_BS(11) XRS_BS(12)
-#undef XRS_BS
-    }
-    if (r2 == kBoxNotTaken) return false;     // TMA cannot describe the raster: the tiled kernels take it
-    *rc = r2;
-    return true;
+// Calls f(std::integral_constant<int, R>{}) with R = rx for rx in 1 .. 12 (the first R tried is R0); false for any
+// other rx.
+template <int R0 = 1, typename F> static bool with_radius(int rx, F &&f) {
+    if constexpr (R0 > kBsMaxK / 2) return false;
+    else return rx == R0 ? f(std::integral_constant<int, R0>{}) : with_radius<R0 + 1>(rx, f);
 }
 
-// focal.apply(mean) over an all-ones kh x kw window (the reference's own focal benchmark, benchmarks/focal.py
-// FocalApply): the same running box in NaN-skipping mode.  true when it took the job (*rc = its status)
-bool try_box_nanmean(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
-                     int kh, int kw, cudaStream_t s, int *rc) {
+bool try_running_box(BoxMode mode, double w, const float *in, int64_t in_pitch, float *out, int64_t out_pitch,
+                     int64_t H, int64_t W, int kh, int kw, cudaStream_t s, int *rc) {
     if (kh > kBsMaxK || kw > kBsMaxK || kh < 1 || kw < 3 || (kw & 1) == 0 || (kh & 1) == 0) return false;
     if (W % 4 != 0 || out_pitch % 16 != 0 || (reinterpret_cast<uintptr_t>(out) & 15)) return false;
     if (H >= (1LL << 31) - 64 || W >= (1LL << 31) - 4096) return false;
-    const double w = 1.0 / (double)(kh * kw);
-    int r2 = kBoxNotTaken;
-    switch (kw / 2) {
-#define XRS_BS(R) case R: r2 = launch_box_stream2<R, kBsWarps, 1>(in, in_pitch, out, out_pitch, H, W, kh, w, s); break;
-        XRS_BS(1) XRS_BS(2) XRS_BS(3) XRS_BS(4) XRS_BS(5) XRS_BS(6) XRS_BS(7) XRS_BS(8) XRS_BS(9) XRS_BS(10) XRS_BS(11) XRS_BS(12)
-#undef XRS_BS
-    }
-    if (r2 == kBoxNotTaken) return false;
-    *rc = r2;
-    return true;
+    return with_radius(kw / 2, [&](auto R) {
+        CUtensorMap tmap;
+        if (!make_tensor_map_2d(&tmap, in, in_pitch, H, W, XRS_F32, BoxShape<R, kBsWarps>::kBoxW, kBoxRows))
+            return false;   // TMA cannot describe the raster: the tiled kernels take it
+        *rc = mode == BoxMode::kConvolve
+                  ? launch_box_stream<R, BoxConvolve>(tmap, in, in_pitch, out, out_pitch, H, W, kh, w, s)
+                  : launch_box_stream<R, BoxNanMean>(tmap, in, in_pitch, out, out_pitch, H, W, kh, w, s);
+        return true;
+    });
 }
 
 }  // namespace xrs

@@ -59,6 +59,13 @@ LaunchInfo &last_launch_info();
 // statistics (conv.cu)
 int check_window(int kh, int kw);
 
+// The running box (box_stream.cu), O(1) work per cell for any window: convolve_2d with every tap the weight w, or
+// focal.apply's mean over an all-ones window (w = 1 / (kh kw)).  Returns false without launching when it cannot
+// take the window (odd sides, kh <= 25, 3 <= kw <= 25) or the raster; otherwise *rc is the launch's status.
+enum class BoxMode { kConvolve, kNanMean };
+bool try_running_box(BoxMode mode, double w, const float *in, int64_t in_pitch, float *out, int64_t out_pitch,
+                     int64_t H, int64_t W, int kh, int kw, cudaStream_t s, int *rc);
+
 // cached per-device properties
 int sm_count(int device = -1);
 

@@ -910,12 +910,6 @@ using namespace xrs;
 int xrs_conv3_strip(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
                     const double *kernel, cudaStream_t s);  // surface.cu
 namespace xrs {
-bool try_box_stream(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
-                    const double *kernel, int kh, int kw, cudaStream_t s, int *rc);
-// box_stream.cu, NaN-skipping mode: focal.apply mean over an all-ones window
-bool try_box_nanmean(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
-                     int kh, int kw, cudaStream_t s, int *rc);  // box_stream.cu
-
 // The focal statistics of one raster: stat is one xrs_focal_stat, written to planes.p[stat], or kAllStats for
 // every plane that is set.  A wide window takes the ring kernel; a single mean over an all-ones window the running
 // box; a raster TMA can describe the tiled kernel, one launch for all the planes; any other raster the
@@ -925,10 +919,11 @@ static int focal_stats(const float *in, int64_t in_pitch, const StatPlanes &plan
     if (is_wide(kh, kw)) return focal_wide(in, in_pitch, planes, out_pitch, H, W, kernel, kh, kw, stat, s);
     static thread_local MaskBits mask;
     const bool all_ones = mask_bits(mask, kernel, kh, kw);
-    if (stat == XRS_STAT_MEAN && all_ones) {  // np.ones((k, k)): the running box, O(1) per cell
-        int brc = XRS_OK;
-        if (try_box_nanmean(in, in_pitch, planes.p[stat], out_pitch, H, W, kh, kw, s, &brc)) return brc;
-    }
+    int brc;
+    if (stat == XRS_STAT_MEAN && all_ones &&   // np.ones((k, k))
+        try_running_box(BoxMode::kNanMean, 1.0 / (double)(kh * kw), in, in_pitch, planes.p[stat], out_pitch, H, W, kh,
+                        kw, s, &brc))
+        return brc;
     float *out = nullptr;  // any plane: the planes share their alignment
     for (float *p : planes.p)
         if (p) out = p;
@@ -960,11 +955,13 @@ int xrs_convolve2d_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
     if (rc) return rc;
     if (is_wide(kh, kw)) return conv2d_wide(in, in_pitch, out, out_pitch, H, W, kernel, kh, kw, (cudaStream_t)s);
     if (kh == 3 && kw == 3) return xrs_conv3_strip(in, in_pitch, out, out_pitch, H, W, kernel, (cudaStream_t)s);
-    {
-        int brc = XRS_OK;
-        // all taps bitwise equal, k <= 25 per side, TMA-describable raster: streaming running-box kernel
-        if (try_box_stream(in, in_pitch, out, out_pitch, H, W, kernel, kh, kw, (cudaStream_t)s, &brc)) return brc;
-    }
+    const double w = kernel[0];   // all taps bitwise equal to a finite w (np.ones((k, k)) / k**2): the running box
+    bool uniform = fabs(w) <= 1.7976931348623157e308;
+    for (int i = 1; uniform && i < kh * kw; ++i) uniform = memcmp(&kernel[i], &w, sizeof(double)) == 0;
+    int brc;
+    if (uniform &&
+        try_running_box(BoxMode::kConvolve, w, in, in_pitch, out, out_pitch, H, W, kh, kw, (cudaStream_t)s, &brc))
+        return brc;
     static thread_local ConvWeights cw;
     for (int i = 0; i < kh * kw; ++i) cw.w[i] = kernel[i];
     TileGeom g;
