@@ -326,6 +326,90 @@ def test_crosstab_3d_var_std_far_from_the_pivot(xb):
             assert (err <= tol).all(), "%s layer %g: worst err/tol %.3g" % (agg, c, (err / tol).max())
 
 
+def test_crosstab_3d_columns_are_zonal_stats_of_their_layers(xb, monkeypatch):
+    """Every category column of a 3-D crosstab is zonal.stats of that layer with the same zone_ids and nodata,
+    its zones in the caller's order with repeats kept.  Layers of float32, float64, float16 and int32 values,
+    one of them with zones far from the pivot (the float32 one takes the second pass over a selection), and a zone
+    without valid cells (in the int32 raster, with nodata only).  min / max / majority and count exactly, the
+    moments within the tolerances of this module: the float64 sums are merged by atomics, so two calls may
+    differ in the last bits."""
+    from xrspatial_b200 import _lib
+    rng = np.random.default_rng(19)
+    h, w = 300, 420
+    y, x = np.mgrid[0:h, 0:w]
+    zones = ((y // 15) * 20 + x // 21).astype(np.int32)                            # 400 zones
+    ids = np.unique(zones)
+    empty, nodata = ids[7], 5.0
+    offs = np.array([0.0, 1e4, 1e6, 1e7, 3e5])                                     # as in the test above
+    base = np.stack([np.round(rng.standard_normal((h, w)) * 160) / 4,              # quarter steps: repeated values
+                     offs[zones % len(offs)] + 0.1 * rng.standard_normal((h, w)),
+                     rng.integers(0, 9, (h, w)).astype(np.float64)])
+    sprinkle = rng.random(base.shape) < 0.05
+    sprinkle[1] = False                                          # nodata cells would widen the far zones' spread
+    base[sprinkle] = nodata
+    base[rng.random(base.shape) < 0.01] = np.nan
+    base[:, zones == empty] = np.nan
+    zagg = xb.DataArray(dev(zones), dims=("y", "x"))
+    cats = [1.0, 2.0, 3.0]
+    aggs = ("mean", "max", "min", "sum", "std", "var", "count", "majority")
+    real_call = _lib.call
+    for dt in (np.float32, np.float64, np.float16, np.int32):
+        with np.errstate(over="ignore"):                        # float16: the offsets above 65504 become inf
+            v3 = (np.where(np.isnan(base), nodata, base) if dt == np.int32 else base).astype(dt)
+        vagg = xb.DataArray(dev(v3), dims=("band", "y", "x"))
+        vagg["band"] = cats
+        for zone_ids in (None, [ids[50], ids[3], empty, ids[50], 10 ** 6, ids[399], ids[0]]):
+            want_zones = ids if zone_ids is None else np.array([z for z in zone_ids if z in ids])
+            df = xb.zonal_crosstab(zagg, vagg, zone_ids=zone_ids, layer=0, cat_ids=[])
+            assert list(df.columns) == ["zone"]
+            np.testing.assert_array_equal(np.asarray(df["zone"]), want_zones)
+            for nd in (None, nodata):
+                what = "%s zone_ids %s nodata %s" % (np.dtype(dt).name, zone_ids is not None, nd)
+                layers = [xb.DataArray(dev(v3[j]), dims=("y", "x")) for j in range(len(cats))]
+                mm = [xb.zonal_stats(zagg, la, zone_ids=zone_ids, stats_funcs=["min", "max", "count"],
+                                     nodata_values=nd) for la in layers]
+                for agg in aggs:
+                    calls = []
+                    monkeypatch.setattr(_lib, "call", lambda name, *a: (calls.append(name), real_call(name, *a))[1])
+                    ct = xb.zonal_crosstab(zagg, vagg, zone_ids=zone_ids, layer=0, agg=agg, nodata_values=nd)
+                    monkeypatch.setattr(_lib, "call", real_call)
+                    if dt == np.float32 and agg == "var" and zone_ids is not None:
+                        assert "xrs_zonal_hash_second_pass" in calls, what
+                    assert list(ct.columns) == ["zone"] + cats, what
+                    zone = np.asarray(ct["zone"])
+                    np.testing.assert_array_equal(zone, want_zones, err_msg=what)
+                    for j, c in enumerate(cats):
+                        st = xb.zonal_stats(zagg, layers[j], zone_ids=zone_ids, stats_funcs=[agg], nodata_values=nd)
+                        row = np.searchsorted(np.asarray(st["zone"]), zone)
+                        np.testing.assert_array_equal(np.asarray(st["zone"])[row], zone, err_msg=what)
+                        t = np.asarray(st[agg], dtype=np.float64)[row]
+                        g = np.asarray(ct[c])
+                        msg = "%s %s layer %g" % (what, agg, c)
+                        if agg == "count":
+                            assert g.dtype == np.int64, msg
+                            np.testing.assert_array_equal(g, np.where(np.isnan(t), 0, t).astype(np.int64), err_msg=msg)
+                            continue
+                        if agg in ("min", "max", "majority"):
+                            np.testing.assert_array_equal(g, t, err_msg=msg)
+                            continue
+                        np.testing.assert_array_equal(np.isnan(g), np.isnan(t), err_msg=msg)
+                        have = ~np.isnan(t)
+                        ref = mm[j]
+                        big = np.maximum(np.abs(np.asarray(ref["min"])), np.abs(np.asarray(ref["max"])))[row][have]
+                        n = np.asarray(ref["count"], dtype=np.float64)[row][have]
+                        g, t = g[have], t[have]
+                        if agg == "mean":
+                            tol = 1e-10 * (np.abs(t) + big)
+                        elif agg == "sum":
+                            tol = 1e-10 * (np.abs(t) + n * big)
+                        else:
+                            if agg == "std":
+                                g, t = g ** 2, t ** 2
+                            tol = 1e-7 * t + 1e-12 * big * big
+                        err = np.abs(g - t)
+                        assert (err <= tol).all(), "%s: worst err/tol %.3g" % (msg, (err / tol).max())
+
+
 # ----------------------------------------------------------------- hotspots
 def classify(z):
     t = dev(np.asarray(z, np.float32))

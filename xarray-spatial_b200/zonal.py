@@ -33,16 +33,38 @@ def _device_tensor(a):
     return as_device_tensor(a)
 
 
-def _prepare(t, allow):
-    """Cast a device tensor to a dtype the kernel reads natively."""
+def _prepare_zones(t):
+    """Zone ids as the contiguous int32, int64, float32 or float64 tensor the kernels read: narrower integers and
+    bool widen to int32, wider unsigned integers to int64, other floating types to float32."""
     import torch
-    if t.dtype in allow:
+    if t.dtype in (torch.int32, torch.int64, torch.float32, torch.float64):
         return t.contiguous()
     if t.dtype.is_floating_point:
-        return t.to(torch.float64 if t.dtype == torch.float64 else torch.float32).contiguous()
+        return t.to(torch.float32).contiguous()
     if t.dtype in (torch.int8, torch.int16, torch.uint8, torch.bool):
         return t.to(torch.int32).contiguous()
     return t.to(torch.int64).contiguous()
+
+
+def _prepare_values(t):
+    """Values as the contiguous float32 or float64 tensor the kernels read: float32 and float64 as they are, other
+    floating types as float32, integers and bool as float64."""
+    import torch
+    if t.dtype in (torch.float32, torch.float64):
+        return t.contiguous()
+    return t.to(torch.float32 if t.dtype.is_floating_point else torch.float64).contiguous()
+
+
+def _select_zones(present, zone_ids, keep_order=False):
+    """(ids, pos): the zones a call reports and their positions in `present`, the sorted ids of the zones found in
+    the raster.  Without `zone_ids`, every present zone, and `pos` is a slice, so that indexing with it copies
+    nothing.  Otherwise the listed ids that are present: sorted and unique (zonal.stats), or in the caller's order
+    with repeats kept when `keep_order` (crosstab).  `z in ndarray` compares with ==, so a NaN id never matches."""
+    if zone_ids is None:
+        return present, slice(None)
+    listed = zone_ids if keep_order else np.unique(zone_ids)
+    ids = np.array([z for z in listed if z in present], dtype=present.dtype)
+    return ids, np.searchsorted(present, ids)
 
 
 _EMPTY_KEY = -(1 << 63)
@@ -472,13 +494,13 @@ def finalize(part, pivot, stats_funcs):
     return cols
 
 
-def _partial_columns(zt, vt, table, ids, part, pivot, names, nodata_values, comm, pos=None):
-    """finalize(...) of `names` over the zones ids[pos] (all `ids` when pos is None) from hash_partials' results.
+def _partial_columns(zt, vt, table, ids, part, pivot, names, nodata_values, comm, pos):
+    """finalize(...) of `names` over the zones ids[pos] from hash_partials' results.
     mean / sum / std / var come from a second pass about each zone's own mean (numpy's two-pass statistics) for
     float64 rasters when std / var are asked for, and whenever the one-pass sums over these zones may be too
     inaccurate (zones far from the pivot for their spread)."""
     import torch
-    sel_part = part if pos is None else {n: a[pos] for n, a in part.items()}
+    sel_part = {n: a[pos] for n, a in part.items()}
     sel_pivot = np.full(len(sel_part["count"]), pivot)
     moments = [s for s in names if s in ("mean", "sum", "std", "var")]
     second = len(sel_pivot) > 0 and bool(moments) and \
@@ -490,57 +512,54 @@ def _partial_columns(zt, vt, table, ids, part, pivot, names, nodata_values, comm
         with np.errstate(invalid="ignore", divide="ignore"):
             means = np.where(cnt > 0, pivot + part["s1"] / cnt, 0.0)
         part2 = second_pass_partials(zt, vt, table, ids, means, nodata_values, comm=comm)
-        if pos is not None:
-            part2 = {n: a[pos] for n, a in part2.items()}
-            means = means[pos]
-        cols.update(finalize(part2, means, moments))
+        cols.update(finalize({n: a[pos] for n, a in part2.items()}, means[pos], moments))
     return cols
+
+
+def _zone_columns(zt, vt, names, nodata_values, comm, zone_ids, keep_order=False):
+    """(ids, cols): the zones `_select_zones(..., zone_ids, keep_order)` reports for the prepared zones `zt` and
+    values `vt`, and one float64 column per built-in statistic of `names`, aligned with them."""
+    table = {}
+    present, part, pivot = hash_partials(zt, vt, nodata_values, comm=comm, table=table)
+    ids, pos = _select_zones(present, zone_ids, keep_order)
+    cols = _partial_columns(zt, vt, table, present, part, pivot, [s for s in names if s != "majority"],
+                            nodata_values, comm, pos)
+    if "majority" in names:
+        cols["majority"] = majority_by_zone(zt, vt, present, nodata_values, comm=comm)[pos]
+    return ids, cols
+
+
+def _zone_table(ids, cols, names, zt, values, return_type):
+    """A zone column and one column per name as a DataFrame, or, for any other `return_type`, every column
+    broadcast back onto its zone's cells in the container of `values`."""
+    if return_type == 'pandas.DataFrame':
+        return pd.DataFrame({"zone": ids, **{s: cols[s] for s in names}})
+    return like_container(_broadcast_back(cols, names, ids, zt), values)
 
 
 def _stats_device(zones, values, zone_ids, stats_funcs, nodata_values, return_type='pandas.DataFrame',
                   comm=None):
     """Device runner (replaces zonal.py:335 `_stats_cupy`)."""
-    import torch
-    zt = _prepare(as_device_tensor(zones), (torch.int32, torch.int64, torch.float32, torch.float64))
-    vt = _prepare(as_device_tensor(values), (torch.float32, torch.float64))
-    if vt.dtype not in (torch.float32, torch.float64):
-        vt = vt.to(torch.float64)
+    zt = _prepare_zones(as_device_tensor(zones))
+    vt = _prepare_values(as_device_tensor(values))
     if len(vt.shape) > 2:
         raise TypeError('3D inputs not supported for the device backend')
     names = list(stats_funcs)
-    table = {}
-    unique_zones, part_all, pivot0 = hash_partials(zt, vt, nodata_values, comm=comm, table=table)
-    if zone_ids is None:
-        sel, pos = unique_zones, None
-    else:
-        sel = np.array([z for z in np.unique(zone_ids) if z in unique_zones], dtype=unique_zones.dtype)
-        pos = np.searchsorted(unique_zones, sel)
-    cols = _partial_columns(zt, vt, table, unique_zones, part_all, pivot0, [s for s in names if s != "majority"],
-                            nodata_values, comm, pos)
-    if "majority" in names:
-        maj = majority_by_zone(zt, vt, unique_zones, nodata_values, comm=comm)
-        cols["majority"] = maj if pos is None else maj[pos]
-    if return_type == 'pandas.DataFrame':
-        d = {"zone": sel}
-        for s in names:
-            d[s] = cols[s]
-        return pd.DataFrame(d)
-    out = _broadcast_back(cols, names, sel, zt, vt.shape, vt.device)
-    return like_container(out, values)
+    ids, cols = _zone_columns(zt, vt, names, nodata_values, comm, zone_ids)
+    return _zone_table(ids, cols, names, zt, values, return_type)
 
 
-def _broadcast_back(cols, names, sel, zt, shape, device):
+def _broadcast_back(cols, names, sel, zt):
     """(len(names), H, W) float64 tensor: every statistic broadcast onto its zone's cells, NaN
     elsewhere (zonal.py:313-331)."""
     import torch
-    H, W = shape
-    out = torch.full((len(names), H * W), float("nan"), dtype=torch.float64, device=device)
+    out = torch.full((len(names), zt.numel()), float("nan"), dtype=torch.float64, device=zt.device)
     if len(sel):
         idx, hit = _zone_index(zt.reshape(-1), sel)
         for i, s in enumerate(names):
-            table = torch.as_tensor(np.asarray(cols[s], dtype=np.float64), device=device)
+            table = torch.as_tensor(np.asarray(cols[s], dtype=np.float64), device=zt.device)
             out[i] = torch.where(hit, table[idx], out[i])
-    return out.reshape(len(names), H, W)
+    return out.reshape(len(names), *zt.shape)
 
 
 def _stats_custom(zones, values, zone_ids, stats_funcs, nodata_values, return_type='pandas.DataFrame',
@@ -551,7 +570,7 @@ def _stats_custom(zones, values, zone_ids, stats_funcs, nodata_values, return_ty
     sort; the callables receive the zone's values in the raster's dtype -- numpy arrays for numpy
     rasters (`host`), device tensors otherwise -- and must return a scalar."""
     import torch
-    zt = _prepare(as_device_tensor(zones), (torch.int32, torch.int64, torch.float32, torch.float64))
+    zt = _prepare_zones(as_device_tensor(zones))
     vt = as_device_tensor(values).contiguous()
     if len(vt.shape) > 2:
         raise TypeError('3D inputs not supported for the device backend')
@@ -561,11 +580,7 @@ def _stats_custom(zones, values, zone_ids, stats_funcs, nodata_values, return_ty
     z = zt.reshape(-1)
     v = vt.reshape(-1)
     zfinite = torch.isfinite(z) if z.dtype.is_floating_point else None
-    unique_zones = torch.unique(z[zfinite] if zfinite is not None else z).cpu().numpy()
-    if zone_ids is None:
-        sel = unique_zones
-    else:
-        sel = np.array([zz for zz in np.unique(zone_ids) if zz in unique_zones], dtype=unique_zones.dtype)
+    sel, _ = _select_zones(torch.unique(z[zfinite] if zfinite is not None else z).cpu().numpy(), zone_ids)
     ok = torch.isfinite(v) if v.dtype.is_floating_point else torch.ones_like(v, dtype=torch.bool)
     if nodata_values is not None:
         ok &= v != nodata_values
@@ -587,13 +602,7 @@ def _stats_custom(zones, values, zone_ids, stats_funcs, nodata_values, return_ty
                 a, b = where[zz]
                 col[i] = float(func(groups[a:b]))
         cols[name] = col
-    names = list(stats_funcs.keys())
-    if return_type == 'pandas.DataFrame':
-        d = {"zone": sel}
-        d.update({n: cols[n] for n in names})
-        return pd.DataFrame(d)
-    out = _broadcast_back(cols, names, sel, zt, vt.shape, vt.device)
-    return out.cpu().numpy() if host else like_container(out, values)
+    return _zone_table(sel, cols, list(stats_funcs), zt, values, return_type)
 
 
 def _stats_host(zones, values, zone_ids, stats_funcs, nodata_values, return_type='pandas.DataFrame'):
@@ -603,10 +612,9 @@ def _stats_host(zones, values, zone_ids, stats_funcs, nodata_values, return_type
         res = _stats_custom(zt, vt, zone_ids, stats_funcs, nodata_values, return_type, host=True)
     else:
         res = _stats_device(zt, vt, zone_ids, stats_funcs, nodata_values, return_type)
-        if return_type != 'pandas.DataFrame':
-            res = res.cpu().numpy()
-    if return_type == 'pandas.DataFrame':
-        res["zone"] = res["zone"].astype(np.asarray(zones).dtype)
+    if return_type != 'pandas.DataFrame':
+        return res.cpu().numpy()
+    res["zone"] = res["zone"].astype(np.asarray(zones).dtype)
     return res
 
 
@@ -708,7 +716,7 @@ def _pivot_pairs(sel, cats, pz, pv, pc):
 def _crosstab_3d(zones, values, zone_ids, cat_ids, layer, agg, nodata_values, comm):
     """3-D `values` (zonal.py:1096-1116, `_single_zone_crosstab_3d` :734-745): the categories are the
     coordinate values of dimension `layer`, and cell (zone, category) is statistic `agg` of that
-    category's 2-D layer over the zone -- i.e. one zonal.stats pass per selected layer."""
+    category's 2-D layer over the zone: the column is zonal.stats of that layer, zones in the order of `zone_ids`."""
     import torch
     if agg not in _DEFAULT_STATS:
         raise ValueError("`agg` method for 3D numpy backed data array must be one of following %s"
@@ -727,37 +735,24 @@ def _crosstab_3d(zones, values, zone_ids, cat_ids, layer, agg, nodata_values, co
     zt = _device_tensor(zones.data)
     if tuple(zt.shape) != tuple(vt.shape[1:]):
         raise ValueError("Incompatible shapes")
-    zt = _prepare(zt, (torch.int32, torch.int64, torch.float32, torch.float64))
+    zt = _prepare_zones(zt)
     if cat_ids is None:
         cats = list(unique_cats.tolist())
     else:
         cats = [c for c in cat_ids if c in unique_cats]
     cat_pos = {c: j for j, c in enumerate(unique_cats.tolist())}
-    zf = zt.reshape(-1)
-    zfin = zf[torch.isfinite(zf)] if zf.dtype.is_floating_point else zf
-    unique_zones = torch.unique(zfin).cpu().numpy()
-    if zone_ids is None:
-        sel = unique_zones
-    else:
-        sel = np.array([z for z in zone_ids if z in unique_zones], dtype=unique_zones.dtype)
-    d = {"zone": sel}
+    d = {}
     for c in cats:
-        lt = vt[cat_pos[c]].contiguous()
-        lt = lt if lt.dtype in (torch.float32, torch.float64) else lt.to(torch.float64)
-        table = {}
-        ids, part, pivot0 = hash_partials(zt, lt, nodata_values, comm=comm, table=table)
-        pos = np.searchsorted(ids, sel)
-        pos = np.clip(pos, 0, max(len(ids) - 1, 0))
-        hit = (ids[pos] == sel) if len(ids) else np.zeros(len(sel), bool)
-        if agg == "majority":
-            col_all = majority_by_zone(zt, lt, ids, nodata_values, comm=comm)
-        else:
-            col_all = _partial_columns(zt, lt, table, ids, part, pivot0, [agg], nodata_values, comm)[agg]
-        col = np.where(hit, col_all[pos] if len(ids) else np.nan, np.nan)
+        ids, cols = _zone_columns(zt, _prepare_values(vt[cat_pos[c]]), [agg], nodata_values, comm, zone_ids,
+                                  keep_order=True)
+        col = cols[agg]
         if agg == "count":          # np.ma.count of an empty selection is 0, and the column is integer
             col = np.where(np.isnan(col), 0, col).astype(np.int64)
         d[c] = col
-    return pd.DataFrame(d)
+    if not cats:                    # the zones alone: every zone is met, even by a pass without valid values
+        ids, _ = _zone_columns(zt, torch.full(zt.shape, float("nan"), device=zt.device), [], None, comm, zone_ids,
+                               keep_order=True)
+    return pd.DataFrame({"zone": ids, **d})
 
 
 def crosstab(zones, values, zone_ids=None, cat_ids=None, layer=None, agg="count", nodata_values=None, comm=None):
@@ -778,11 +773,9 @@ def crosstab(zones, values, zone_ids=None, cat_ids=None, layer=None, agg="count"
     validate_arrays(zones, values)
     if agg not in ("percentage", "count"):
         raise ValueError("`agg` method for 2D data array must be one of following ['percentage', 'count']")
-    import torch
-    zt, vt = _device_tensor(zones.data), _device_tensor(values.data)
-    zt = _prepare(zt, (torch.int32, torch.int64, torch.float32, torch.float64))
-    vt_f = vt.contiguous() if vt.dtype in (torch.float32, torch.float64) else vt.to(torch.float64)
-    unique_zones, _, _ = hash_partials(zt, vt_f, None, comm=comm)
+    zt, vt = _prepare_zones(_device_tensor(zones.data)), _device_tensor(values.data)
+    vt_f = _prepare_values(vt)
+    present, _, _ = hash_partials(zt, vt_f, None, comm=comm)
     zi, vf = _pair_inputs(zt, vt_f)
     try:
         pz, pv, pc = pair_counts(zi, vf, nodata_values, comm=comm)
@@ -794,10 +787,7 @@ def crosstab(zones, values, zone_ids=None, cat_ids=None, layer=None, agg="count"
         cats = unique_cats
     else:
         cats = [c for c in cat_ids if c in unique_cats]
-    if zone_ids is None:
-        sel = unique_zones
-    else:
-        sel = np.array([z for z in zone_ids if z in unique_zones], dtype=unique_zones.dtype)
+    sel, _ = _select_zones(present, zone_ids, keep_order=True)
     cats = sorted(cats)
     total, counts = _pivot_pairs(sel, cats, pz, pv, pc)
     table = {c: counts[j] for j, c in enumerate(cats)}
