@@ -5,7 +5,7 @@
 //      register stores (st.global.cs.v4) and the bulk-store epilogue (staging in shared memory, one
 //      cp.async.bulk per tile row issued by a store warp);
 //  (2) the flagship operators (square-cell slope, hillshade, focal.mean f32) over ROWS x STAGES x WARPS x
-//      CTAs per SM with both epilogues, then the other users of surface.cu's XRS_CFG_* geometries;
+//      CTAs per SM with both epilogues, then the other float32 operators of surface.cu's geometry();
 //  (1c) where the input boxes start: the shipped 32-byte halo (every box row starts on an L2 sector) against
 //      a 16-byte halo (every float32 box row starts 16 B into a sector), alternating, for the no-op operator and
 //      the flagship three and the 4-output suite; as the control, a float64 copy with its 32-byte halo read from an aligned base and
@@ -313,7 +313,7 @@ int main(int argc, char **argv) {
         SWEEP("hillshade", HillshadeOp, hp)
         SWEEP("focal.mean f32", FM, fp)
 
-        // ---- (2b) the other users of XRS_CFG_*
+        // ---- (2b) the other float32 operators of surface.cu's geometry()
 #define OTHER(NAME, OP, IN, OUT, HH, PRM, BYTES) { size_t a = smi.mark(); \
             BOTH(NAME, OP, IN, OUT, HH, PRM, 2, 4, 16, 1, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 3, 8, 2, BYTES) \
             BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 4, 8, 1, BYTES) BOTH(NAME, OP, IN, OUT, HH, PRM, 4, 3, 16, 1, BYTES) \

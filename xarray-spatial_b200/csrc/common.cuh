@@ -59,6 +59,12 @@ LaunchInfo &last_launch_info();
 // statistics (conv.cu)
 int check_window(int kh, int kw);
 
+// Slope, aspect, curvature or hillshade (op 0-3, an xrs_op) on a device raster of in_dtype cells: float32, or
+// int16 / uint16 / int32 / float64 converted in registers; float32 out (surface.cu).  p: slope {csx, csy};
+// curvature {cellsize}; hillshade {azimuth, altitude}; aspect takes none.
+int surface_op(int op, const void *in, int in_dtype, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H,
+               int64_t W, const double *p, cudaStream_t s);
+
 // The running box (box_stream.cu), O(1) work per cell for any window: convolve_2d with every tap the weight w, or
 // focal.apply's mean over an all-ones window (w = 1 / (kh kw)).  Returns false without launching when it cannot
 // take the window (odd sides, kh <= 25, 3 <= kw <= 25) or the raster; otherwise *rc is the launch's status.

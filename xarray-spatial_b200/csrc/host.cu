@@ -80,7 +80,7 @@ static int host_op_shape(int op, int in_dtype, const double *p, const double *au
         case XRS_OP_HILLSHADE:
             XRS_REQUIRE(p || op == XRS_OP_ASPECT, "scalar parameters missing");
             if (in_dtype == XRS_F32) return XRS_OK;
-            // raw cells go to the direct-ingest TMA kernels (xrs_surface_typed), which need W % 4 == 0
+            // raw cells go to the direct-ingest TMA kernels (surface_op), which need W % 4 == 0
             XRS_REQUIRE(in_dtype == XRS_F64 || in_dtype == XRS_I32 || in_dtype == XRS_I16 || in_dtype == XRS_U16,
                         "in_dtype must be float32, int16, uint16, int32 or float64");
             XRS_REQUIRE(W % 4 == 0, "int16 / uint16 / int32 / float64 host input needs W % 4 == 0");
@@ -103,15 +103,13 @@ static int host_op_shape(int op, int in_dtype, const double *p, const double *au
 
 static int run_op(int op, int in_dtype, const void *din, void *dout, int64_t pitch, int64_t opitch, int64_t h,
                   int64_t W, const double *p, const double *aux, int naux, cudaStream_t s) {
-    if (in_dtype != XRS_F32 && op != XRS_OP_FOCAL_MEAN)  // raw int16 / uint16 / int32 / float64 cells
-        return xrs_surface_typed(op, din, in_dtype, pitch, (float *)dout, opitch, h, W, p, s);
     const float *fi = (const float *)din;
     float *fo = (float *)dout;
     switch (op) {
-        case XRS_OP_SLOPE: return xrs_slope_f32(fi, pitch, fo, opitch, h, W, p[0], p[1], s);
-        case XRS_OP_ASPECT: return xrs_aspect_f32(fi, pitch, fo, opitch, h, W, s);
-        case XRS_OP_CURVATURE: return xrs_curvature_f32(fi, pitch, fo, opitch, h, W, p[0], s);
-        case XRS_OP_HILLSHADE: return xrs_hillshade_f32(fi, pitch, fo, opitch, h, W, p[0], p[1], s);
+        case XRS_OP_SLOPE:
+        case XRS_OP_ASPECT:
+        case XRS_OP_CURVATURE:
+        case XRS_OP_HILLSHADE: return surface_op(op, din, in_dtype, pitch, fo, opitch, h, W, p, s);
         case XRS_OP_FOCAL_MEAN:
             if (in_dtype == XRS_F64)
                 return xrs_focal_mean_f64((const double *)din, pitch, (double *)dout, opitch, h, W, aux, naux, s);

@@ -588,15 +588,19 @@ bool strip_tma_map(CUtensorMap *map, const TS *in, int64_t in_pitch_bytes, int64
 
 constexpr int kFallbackRows = 4, kFallbackStages = 4;  // cp.async ring (per warp)
 
-template <typename Op, int ROWS, int STAGES, int WARPS = 8, int CTAS = 2>
-int launch_stencil3(const typename Op::in_t *in, int64_t in_pitch_bytes, const typename Op::Params &prm,
+// Checks the arguments, then runs the TMA kernel when strip_tma_map takes the raster, else the cp.async kernel.
+// TS is the cell type in HBM: for TS != Op::in_t (int16 / uint16 / int32 / float64 cells converted in registers)
+// only the TMA kernel exists, and other layouts return XRS_EUNSUPPORTED.
+template <typename Op, int ROWS, int STAGES, int WARPS, int CTAS, typename TS = typename Op::in_t>
+int launch_stencil3(const TS *in, int64_t in_pitch_bytes, const typename Op::Params &prm,
                     typename Op::out_t *const *out_ptrs, int64_t out_pitch_bytes, int64_t H, int64_t W,
                     cudaStream_t stream) {
     using T = typename Op::in_t;
     using TO = typename Op::out_t;
+    constexpr bool kConvert = !std::is_same<TS, T>::value;
     if (H <= 0 || W <= 0) return XRS_OK;  // empty raster: nothing to do
     XRS_REQUIRE(in != nullptr, "input pointer is NULL");
-    XRS_REQUIRE(in_pitch_bytes % (int64_t)sizeof(T) == 0 && in_pitch_bytes >= W * (int64_t)sizeof(T),
+    XRS_REQUIRE(in_pitch_bytes % (int64_t)sizeof(TS) == 0 && in_pitch_bytes >= W * (int64_t)sizeof(TS),
                 "input pitch must be a multiple of the element size and >= row bytes");
     XRS_REQUIRE(out_pitch_bytes % (int64_t)sizeof(TO) == 0 && out_pitch_bytes >= W * (int64_t)sizeof(TO),
                 "output pitch must be a multiple of the element size and >= row bytes");
@@ -617,8 +621,12 @@ int launch_stencil3(const typename Op::in_t *in, int64_t in_pitch_bytes, const t
 
     CUtensorMap tmap;
     if (strip_tma_map(&tmap, in, in_pitch_bytes, H, W, ROWS, out_vec_ok))
-        return launch_tma<Op, ROWS, STAGES, WARPS, CTAS>(tmap, prm, outs, H, W, stream, kStripTma);
-    {  // rasters TMA cannot describe: the per-warp cp.async ring
+        return launch_tma<Op, ROWS, STAGES, WARPS, CTAS, TS>(tmap, prm, outs, H, W, stream,
+                                                             kConvert ? kIngestTma : kStripTma);
+    if constexpr (kConvert) {
+        set_error("raster layout not supported by the direct-ingest path (needs 16-byte aligned rows, W %% 4 == 0)");
+        return XRS_EUNSUPPORTED;
+    } else {  // rasters TMA cannot describe: the per-warp cp.async ring
         constexpr int FR = sizeof(T) == 8 ? 2 : kFallbackRows, FS = kFallbackStages;
         StripGeom g;
         g.H = H;
