@@ -230,6 +230,29 @@ int xrs_zonal_pair_count(const float *values, const int32_t *zones, int64_t n, i
                          int has_nodata, double nodata, int64_t *keys, int64_t *count, int cap,
                          int *overflow, xrs_stream_t s);
 
+/* ------------------------------------------------------------------ proximity
+ * proximity / allocation / direction (proximity.py:401-647) as an exact nearest-target transform: every cell gets
+ * the target nearest to it under the metric, the first in row-major order among equidistant ones (the reference's
+ * GDAL-style sweep only approximates this; DESIGN.md section 4.7).  Rasters of H x W cells of in_dtype (any
+ * xrs_dtype), rows in_pitch bytes apart; x[W] and y[H] are DEVICE float64 coordinates, each strictly ascending
+ * or strictly descending (GREAT_CIRCLE: degrees of longitude / latitude within +-180 / +-90).
+ * targets: NULL for the default rule (nonzero and finite cells), else a DEVICE array of n_targets float64
+ * values sorted ascending without NaN (a cell is a target when its value, widened to float64, is one of them;
+ * n_targets may be 0: no cell is).  float32 output, rows out_pitch bytes apart: the distance
+ * (XRS_PROX_DISTANCE), the nearest target's value (XRS_PROX_ALLOCATION) or the compass direction to it
+ * (XRS_PROX_DIRECTION, 0 on targets); NaN where there is no target or the float32 squared distance exceeds
+ * max_distance^2.
+ * scratch: a DEVICE buffer of at least xrs_proximity_scratch_bytes(H, W, band_rows) bytes (about 8 bytes per
+ * cell); band_rows (0: the library's choice) splits the column pass into bands and does not change the result.
+ * Enqueues on `s` only; a bad argument returns XRS_EINVAL before any CUDA call. */
+enum xrs_metric { XRS_METRIC_EUCLIDEAN = 0, XRS_METRIC_GREAT_CIRCLE = 1, XRS_METRIC_MANHATTAN = 2 };
+enum xrs_prox_mode { XRS_PROX_DISTANCE = 0, XRS_PROX_ALLOCATION = 1, XRS_PROX_DIRECTION = 2 };
+int xrs_proximity_scratch_bytes(int64_t H, int64_t W, int band_rows, int64_t *bytes);
+int xrs_proximity(const void *in, int in_dtype, int64_t in_pitch, int64_t H, int64_t W, const double *x,
+                  const double *y, const double *targets, int n_targets, double max_distance, int metric,
+                  int mode, float *out, int64_t out_pitch, void *scratch, int64_t scratch_bytes, int band_rows,
+                  xrs_stream_t s);
+
 /* ------------------------------------------------------------------ host-buffer (end-to-end)
  * Same operators on HOST rasters: the library cuts the raster into row chunks and overlaps
  * host->device copies, kernels and device->host copies on internal streams.  `op` selects
@@ -265,7 +288,7 @@ int xrs_host_free(void *ptr);
  * mean over an all-ones window), 4 generic tiled convolve, 5 bounds-checked convolve fallback, 6 fused focal
  * statistics, 7 tiled single focal statistic, 8 bounds-checked focal statistic fallback, 9 zonal group-by
  * (xrs_zonal_hash_run / _second_pass), 10 zonal pair count (xrs_zonal_pair_count), 11 wide-window convolve,
- * 12 wide-window single focal statistic, 13 wide-window fused focal statistics -- and with how many CTAs */
+ * 12 wide-window single focal statistic, 13 wide-window fused focal statistics, 14 proximity row pass -- and with how many CTAs */
 int xrs_debug_last_used_tma(void);
 int xrs_debug_last_grid(void);
 /* host-only test hook: the row-segment height the persistent kernels pick for a raster of H rows cut into

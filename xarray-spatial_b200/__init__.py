@@ -12,6 +12,8 @@ from .curvature import curvature  # noqa: F401
 from .focal import apply as focal_apply  # noqa: F401
 from .focal import focal_stats, hotspots, mean  # noqa: F401
 from .hillshade import hillshade  # noqa: F401
+from .proximity import allocation, direction, euclidean_distance, great_circle_distance  # noqa: F401
+from .proximity import manhattan_distance, proximity  # noqa: F401
 from .multispectral import arvi, ebbi, evi, gci, nbr, nbr2, ndmi, ndvi, savi, sipi  # noqa: F401
 from .slope import slope  # noqa: F401
 from .zonal import crosstab as zonal_crosstab  # noqa: F401

@@ -57,6 +57,8 @@ def _declare(lib):
         "xrs_zonal_hash_run": [P, I, P, I, I64, I64, I, D, I, D, P, P, P, P, P, P, I, P, I, P, P],
         "xrs_zonal_hash_second_pass": [P, I, P, I, I64, I64, I, D, P, P, P, P, P, P, P, I, P, I, P, P],
         "xrs_zonal_pair_count": [P, P, I64, I64, I, D, P, P, I, P, P],
+        "xrs_proximity_scratch_bytes": [I64, I64, I, ctypes.POINTER(I64)],
+        "xrs_proximity": [P, I, I64, I64, I64, P, P, P, I, D, I, I, P, I64, P, I64, I, P],
         "xrs_host_stencil": [I, P, I, P, I64, I64, P, P, I, P, I],
         "xrs_host_release": [I],
         "xrs_host_alloc": [ctypes.POINTER(P), I64],

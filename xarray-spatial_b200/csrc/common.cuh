@@ -33,6 +33,7 @@ enum LaunchKind : int {
     kConvWide = 11,     // convolve over a window beyond the tiled kernels (conv.cu, "wide windows")
     kFocalWide = 12,    // single focal statistic over such a window
     kFocalWideFused = 13,  // every requested focal statistic over such a window
+    kProximity = 14,    // proximity / allocation / direction row pass (proximity.cu)
 };
 
 struct LaunchInfo {  // for tests / profiling: what the last launch on this thread chose
