@@ -253,6 +253,20 @@ int xrs_proximity(const void *in, int in_dtype, int64_t in_pitch, int64_t H, int
                   int mode, float *out, int64_t out_pitch, void *scratch, int64_t scratch_bytes, int band_rows,
                   xrs_stream_t s);
 
+/* ------------------------------------------------------------------ viewshed
+ * viewshed (viewshed.py:1122-1502) as a per-cell line-of-sight test that makes the reference sweep's
+ * visible / invisible decision (DESIGN.md section 4.8).  Rasters of H x W cells of in_dtype (any xrs_dtype, read
+ * as float64, never written), rows in_pitch bytes apart; the observer stands on cell (vp_row, vp_col) at
+ * vp_elev; target_elev is added to every cell seen as a target; ew_res / ns_res are the coordinate steps between
+ * columns / rows (may be negative or NaN).  float64 output, rows out_pitch bytes apart: 180 at the observer, the
+ * vertical angle in degrees of a visible cell, -1 otherwise (NaN cells never block and are -1).
+ * scratch: a DEVICE buffer of at least xrs_viewshed_scratch_bytes(H, W) bytes (56 bytes per cell).
+ * Enqueues on `s` only; a bad argument returns XRS_EINVAL before any CUDA call. */
+int xrs_viewshed_scratch_bytes(int64_t H, int64_t W, int64_t *bytes);
+int xrs_viewshed(const void *in, int in_dtype, int64_t in_pitch, int64_t H, int64_t W, int64_t vp_row,
+                 int64_t vp_col, double vp_elev, double target_elev, double ew_res, double ns_res, double *out,
+                 int64_t out_pitch, void *scratch, int64_t scratch_bytes, xrs_stream_t s);
+
 /* ------------------------------------------------------------------ host-buffer (end-to-end)
  * Same operators on HOST rasters: the library cuts the raster into row chunks and overlaps
  * host->device copies, kernels and device->host copies on internal streams.  `op` selects

@@ -59,6 +59,8 @@ def _declare(lib):
         "xrs_zonal_pair_count": [P, P, I64, I64, I, D, P, P, I, P, P],
         "xrs_proximity_scratch_bytes": [I64, I64, I, ctypes.POINTER(I64)],
         "xrs_proximity": [P, I, I64, I64, I64, P, P, P, I, D, I, I, P, I64, P, I64, I, P],
+        "xrs_viewshed_scratch_bytes": [I64, I64, ctypes.POINTER(I64)],
+        "xrs_viewshed": [P, I, I64, I64, I64, I64, I64, D, D, D, D, P, I64, P, I64, P],
         "xrs_host_stencil": [I, P, I, P, I64, I64, P, P, I, P, I],
         "xrs_host_release": [I],
         "xrs_host_alloc": [ctypes.POINTER(P), I64],
