@@ -267,6 +267,32 @@ int xrs_viewshed(const void *in, int in_dtype, int64_t in_pitch, int64_t H, int6
                  int64_t vp_col, double vp_elev, double target_elev, double ew_res, double ns_res, double *out,
                  int64_t out_pitch, void *scratch, int64_t scratch_bytes, xrs_stream_t s);
 
+/* ------------------------------------------------------------------ a_star_search
+ * a_star_search (pathfinding.py:233-382) as an exact shortest-path search (DESIGN.md section 4.9).  Rasters of
+ * H x W cells of in_dtype (any xrs_dtype, read as float64, never written), rows in_pitch bytes apart, H W < 2^31.
+ * A cell is crossable unless it is NaN or equal to one of the n_barriers DEVICE float64 values in `barriers`
+ * (NULL when n_barriers is 0).  Moves go to the 8 neighbours, or 4 with connectivity 4, and cost 1 or sqrt(2).
+ * xrs_a_star_search: float64 output, rows out_pitch bytes apart, NaN except along a shortest path from the start
+ * to the goal, which holds the running sum of the step lengths (0 at the start); all NaN when there is no path.
+ * Among equally short paths it takes, from each cell, the first move of the reference's neighbour order that stays
+ * on a shortest path.  *rounds (may be NULL) receives the number of relaxation rounds.  scratch: a DEVICE buffer
+ * of at least xrs_a_star_scratch_bytes(H, W) bytes (about 9 bytes per cell); after the call it holds, from byte
+ * 256, the field of shortest lengths to the goal as int32 pairs (orthogonal, diagonal steps; INT32_MAX, 0 where
+ * no path reaches), row-major.
+ * xrs_a_star_snap: the cell _find_nearest_pixel picks for (row, col): itself when crossable, else the crossable
+ * cell at the least pixel distance below the raster's diagonal, the first in row-major order among equals; -1, -1
+ * when there is none.  scratch: a DEVICE buffer of at least 256 bytes.
+ * Unlike the other entry points, both SYNCHRONIZE with `s` before they return: the search reads an activity
+ * count every few rounds and the snap returns its cell.  A bad argument returns XRS_EINVAL before any CUDA call. */
+int xrs_a_star_scratch_bytes(int64_t H, int64_t W, int64_t *bytes);
+int xrs_a_star_search(const void *in, int in_dtype, int64_t in_pitch, int64_t H, int64_t W, const double *barriers,
+                      int n_barriers, int connectivity, int64_t start_row, int64_t start_col, int64_t goal_row,
+                      int64_t goal_col, double *out, int64_t out_pitch, void *scratch, int64_t scratch_bytes,
+                      int64_t *rounds, xrs_stream_t s);
+int xrs_a_star_snap(const void *in, int in_dtype, int64_t in_pitch, int64_t H, int64_t W, const double *barriers,
+                    int n_barriers, int64_t row, int64_t col, int64_t *snap_row, int64_t *snap_col, void *scratch,
+                    int64_t scratch_bytes, xrs_stream_t s);
+
 /* ------------------------------------------------------------------ host-buffer (end-to-end)
  * Same operators on HOST rasters: the library cuts the raster into row chunks and overlaps
  * host->device copies, kernels and device->host copies on internal streams.  `op` selects
