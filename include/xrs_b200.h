@@ -293,6 +293,33 @@ int xrs_a_star_snap(const void *in, int in_dtype, int64_t in_pitch, int64_t H, i
                     int n_barriers, int64_t row, int64_t col, int64_t *snap_row, int64_t *snap_col, void *scratch,
                     int64_t scratch_bytes, xrs_stream_t s);
 
+/* ------------------------------------------------------------------ perlin / generate_terrain
+ * perlin (perlin.py:189) and generate_terrain (terrain.py:183) with the reference's NumPy path as the semantics
+ * (DESIGN.md section 4.10).
+ * xrs_perm_tables: for each of the n_seeds (1 .. 32) HOST seeds, writes RandomState(seed).permutation(n) as int32
+ * to `tables` (DEVICE, n_seeds x n, n 1 .. 2^20), bit for bit.  scratch: a DEVICE buffer of at least
+ * xrs_perm_tables_scratch_bytes(n_seeds, n) bytes (about 22 bytes per table entry plus 2 MB per seed).  *rounds
+ * (may be NULL) receives the number of reservation rounds of the shuffle.  It SYNCHRONIZES with `s`: the host reads
+ * how far the draws got and how many steps are pending between batches of launches.
+ * xrs_noise: H x W cells of float32 or float64 (dtype), rows in_pitch / out_pitch bytes apart; `in` (read only for
+ * terrain, never written) and `out` have the same cell type.  terrain 0 is perlin: one octave from tables[0 .. 2^20)
+ * at the float32 DEVICE coordinates xs (W values) and ys (H values), then (d - min) / (max - min).  terrain 1 is
+ * generate_terrain: 16 octaves, octave o from tables[o 2^20 ..) at float32(x 2^o) weighed by 2^-o, added to in 0,
+ * then / 1.97, the cube, the same normalisation, cells below 0.3 set to 0, and the product with zfactor.
+ * index_stats (DEVICE, 5 int32 per octave: a bad-coordinate flag, the least and largest of P[xi] and P[xi + 1] over
+ * the columns, the least and largest yi over the rows) tells the caller whether the reference would index its
+ * doubled table outside [-2^21, 2^21) and raise IndexError; the output is then meaningless.  scratch: a DEVICE
+ * buffer of at least xrs_noise_scratch_bytes(H, W, terrain) bytes (24 bytes per row and column per octave); after
+ * the call its first 16 bytes hold the field's min and max before normalisation, as float64.  Enqueue-only.  A bad argument returns
+ * XRS_EINVAL before any CUDA call. */
+int xrs_perm_tables_scratch_bytes(int n_seeds, int64_t n, int64_t *bytes);
+int xrs_perm_tables(const uint32_t *seeds, int n_seeds, int64_t n, int32_t *tables, void *scratch,
+                    int64_t scratch_bytes, int64_t *rounds, xrs_stream_t s);
+int xrs_noise_scratch_bytes(int64_t H, int64_t W, int terrain, int64_t *bytes);
+int xrs_noise(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W, const int32_t *tables,
+              const float *xs, const float *ys, int terrain, double zfactor, void *out, int64_t out_pitch,
+              int32_t *index_stats, void *scratch, int64_t scratch_bytes, xrs_stream_t s);
+
 /* ------------------------------------------------------------------ host-buffer (end-to-end)
  * Same operators on HOST rasters: the library cuts the raster into row chunks and overlaps
  * host->device copies, kernels and device->host copies on internal streams.  `op` selects

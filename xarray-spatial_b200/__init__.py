@@ -15,8 +15,10 @@ from .hillshade import hillshade  # noqa: F401
 from .proximity import allocation, direction, euclidean_distance, great_circle_distance  # noqa: F401
 from .proximity import manhattan_distance, proximity  # noqa: F401
 from .pathfinding import a_star_search  # noqa: F401
+from .perlin import perlin  # noqa: F401
 from .multispectral import arvi, ebbi, evi, gci, nbr, nbr2, ndmi, ndvi, savi, sipi  # noqa: F401
 from .slope import slope  # noqa: F401
+from .terrain import generate_terrain  # noqa: F401
 from .viewshed import viewshed  # noqa: F401
 from .zonal import crosstab as zonal_crosstab  # noqa: F401
 from .zonal import stats as zonal_stats  # noqa: F401

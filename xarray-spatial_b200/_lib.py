@@ -65,7 +65,11 @@ def _declare(lib):
         "xrs_a_star_search": [P, I, I64, I64, I64, P, I, I, I64, I64, I64, I64, P, I64, P, I64,
                               ctypes.POINTER(I64), P],
         "xrs_a_star_snap": [P, I, I64, I64, I64, P, I, I64, I64, ctypes.POINTER(I64), ctypes.POINTER(I64), P, I64, P],
-        "xrs_host_stencil": [I, P, I, P, I64, I64, P, P, I, P, I],
+        "xrs_perm_tables_scratch_bytes": [I, I64, ctypes.POINTER(I64)],
+        "xrs_perm_tables": [P, I, I64, P, P, I64, ctypes.POINTER(I64), P],
+        "xrs_noise_scratch_bytes": [I64, I64, I, ctypes.POINTER(I64)],
+        "xrs_noise": [P, I, I64, I64, I64, P, P, P, I, D, P, I64, P, P, I64, P],
+        "xrs_host_stencil":[I, P, I, P, I64, I64, P, P, I, P, I],
         "xrs_host_release": [I],
         "xrs_host_alloc": [ctypes.POINTER(P), I64],
         "xrs_host_free": [P],
