@@ -320,6 +320,45 @@ int xrs_noise(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W,
               const float *xs, const float *ys, int terrain, double zfactor, void *out, int64_t out_pitch,
               int32_t *index_stats, void *scratch, int64_t scratch_bytes, xrs_stream_t s);
 
+/* ------------------------------------------------------------------ classify (classify.cu)
+ * Rasters are H x W cells of `dtype` (any xrs_dtype), rows in_pitch bytes apart, read and never written.  A key is
+ * the order-preserving unsigned image of a cell's bits (-0.0 folded into +0.0; 16-, 32- or 64-bit by the cell
+ * type); "finite" is every integer cell and the float cells that are neither NaN nor +-inf.
+ * xrs_classify_cells: member 0 is the reference's _cpu_bin: each finite cell is compared in float64 with bins[nb]
+ * (DEVICE) by its binary search and gets new_values[bin] (DEVICE float32), anything else NaN; float32 out.  member
+ * 1 is _cpu_binary: 1 where the cell equals one of the nb DEVICE float64 values, else 0 (NaN for a non-finite
+ * float cell); out has the cell type.  nb = 0 is allowed.  Enqueue-only.
+ * xrs_classify_moments: out5 (DEVICE float64) = count, mean, M2 (sum of squared deviations), min and max of the
+ * finite cells above `above` (-inf: all of them), each CTA merging in a fixed order.  Enqueue-only.
+ * xrs_classify_select: exact order statistics by 8-bit digit passes from the top of a `bits`-wide key; each pass
+ * reads the source once for every rank.  source 0: the raster's finite cells.  source 1: the gaps of the unique
+ * values of xrs_classify_sort's keys (in: those keys, H = 1, W = their count; the gap at position i is the cell
+ * type's difference of keys i and i - 1 when they differ).  source 2: the positions of the gaps whose key is `tie`.
+ * With nr = 0 it runs the top-digit pass, writes its 256 counts to hist0 (HOST) and the number of keys to
+ * *n_keys; with nr > 0, hist0 must hold those counts, and keys[i] (HOST) gets the ranks[i]-th smallest key
+ * (0-based, HOST ranks) and rem[i] the rank less the keys below that key.  SYNCHRONIZES with `s` every pass.
+ * xrs_classify_sort: the finite cells' keys, sorted ascending by an LSD radix sort, into keys (DEVICE, n_keys
+ * entries of 4 bytes, or 8 for 64-bit keys; room for H W).  SYNCHRONIZES with `s` once, to read the count.
+ * xrs_classify_pick: over n sorted keys, mode 0 writes every unique key (in no order), mode 1 the key pairs
+ * (i - 1, i) of the gaps above key `tie` or equal to it at a position >= pos; at most cap entries (pairs) go to
+ * out (DEVICE), *count gets how many there are.  scratch: 8 bytes.  SYNCHRONIZES with `s`.
+ * A bad argument returns XRS_EINVAL before any CUDA call. */
+int xrs_classify_cells(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W, int member,
+                       const double *bins, const float *new_values, int nb, void *out, int64_t out_pitch,
+                       xrs_stream_t s);
+int xrs_classify_moments_scratch_bytes(int64_t *bytes);
+int xrs_classify_moments(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W, double above,
+                         double *out5, void *scratch, int64_t scratch_bytes, xrs_stream_t s);
+int xrs_classify_select_scratch_bytes(int64_t *bytes);
+int xrs_classify_select(int source, const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W, int bits,
+                        uint64_t tie, const int64_t *ranks, int nr, uint64_t *keys, int64_t *rem, int64_t *n_keys,
+                        uint64_t *hist0, void *scratch, int64_t scratch_bytes, xrs_stream_t s);
+int xrs_classify_sort_scratch_bytes(int64_t n, int dtype, int64_t *bytes);
+int xrs_classify_sort(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W, void *keys, int64_t *n_keys,
+                      void *scratch, int64_t scratch_bytes, xrs_stream_t s);
+int xrs_classify_pick(const void *sorted, int dtype, int64_t n, int mode, uint64_t tie, int64_t pos, void *out,
+                      int64_t cap, int64_t *count, void *scratch, xrs_stream_t s);
+
 /* ------------------------------------------------------------------ host-buffer (end-to-end)
  * Same operators on HOST rasters: the library cuts the raster into row chunks and overlaps
  * host->device copies, kernels and device->host copies on internal streams.  `op` selects
@@ -355,7 +394,7 @@ int xrs_host_free(void *ptr);
  * mean over an all-ones window), 4 generic tiled convolve, 5 bounds-checked convolve fallback, 6 fused focal
  * statistics, 7 tiled single focal statistic, 8 bounds-checked focal statistic fallback, 9 zonal group-by
  * (xrs_zonal_hash_run / _second_pass), 10 zonal pair count (xrs_zonal_pair_count), 11 wide-window convolve,
- * 12 wide-window single focal statistic, 13 wide-window fused focal statistics, 14 proximity row pass -- and with how many CTAs */
+ * 12 wide-window single focal statistic, 13 wide-window fused focal statistics, 14 proximity row pass, 15 classify per-cell pass -- and with how many CTAs */
 int xrs_debug_last_used_tma(void);
 int xrs_debug_last_grid(void);
 /* host-only test hook: the row-segment height the persistent kernels pick for a raster of H rows cut into

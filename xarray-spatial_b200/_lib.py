@@ -69,6 +69,15 @@ def _declare(lib):
         "xrs_perm_tables": [P, I, I64, P, P, I64, ctypes.POINTER(I64), P],
         "xrs_noise_scratch_bytes": [I64, I64, I, ctypes.POINTER(I64)],
         "xrs_noise": [P, I, I64, I64, I64, P, P, P, I, D, P, I64, P, P, I64, P],
+        "xrs_classify_cells": [P, I, I64, I64, I64, I, P, P, I, P, I64, P],
+        "xrs_classify_moments_scratch_bytes": [ctypes.POINTER(I64)],
+        "xrs_classify_moments": [P, I, I64, I64, I64, D, P, P, I64, P],
+        "xrs_classify_select_scratch_bytes": [ctypes.POINTER(I64)],
+        "xrs_classify_select": [I, P, I, I64, I64, I64, I, ctypes.c_uint64, P, I, P, P, ctypes.POINTER(I64), P, P,
+                                I64, P],
+        "xrs_classify_sort_scratch_bytes": [I64, I, ctypes.POINTER(I64)],
+        "xrs_classify_sort": [P, I, I64, I64, I64, P, ctypes.POINTER(I64), P, I64, P],
+        "xrs_classify_pick": [P, I, I64, I, ctypes.c_uint64, I64, P, I64, ctypes.POINTER(I64), P, P],
         "xrs_host_stencil":[I, P, I, P, I64, I64, P, P, I, P, I],
         "xrs_host_release": [I],
         "xrs_host_alloc": [ctypes.POINTER(P), I64],

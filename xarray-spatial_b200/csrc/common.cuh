@@ -34,6 +34,7 @@ enum LaunchKind : int {
     kFocalWide = 12,    // single focal statistic over such a window
     kFocalWideFused = 13,  // every requested focal statistic over such a window
     kProximity = 14,    // proximity / allocation / direction row pass (proximity.cu)
+    kClassify = 15,     // classify per-cell bin / membership pass (classify.cu)
 };
 
 struct LaunchInfo {  // for tests / profiling: what the last launch on this thread chose
