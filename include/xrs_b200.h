@@ -359,6 +359,24 @@ int xrs_classify_sort(const void *in, int dtype, int64_t in_pitch, int64_t H, in
 int xrs_classify_pick(const void *sorted, int dtype, int64_t n, int mode, uint64_t tie, int64_t pos, void *out,
                       int64_t cap, int64_t *count, void *scratch, xrs_stream_t s);
 
+/* ------------------------------------------------------------------ natural_breaks (natural_breaks.cu)
+ * xrs_nb_sample: the set of the first s entries of np.linspace(0, n, n, dtype=uint32) after
+ * RandomState(seed).shuffle -- the reference's sample of cell indices -- in ascending order, as int64 to out
+ * (DEVICE, s entries), for 1 <= s < n <= 2^32 (more cells: XRS_EINVAL).  scratch: a DEVICE buffer of at least
+ * xrs_nb_sample_scratch_bytes(n, s) bytes (about 10 bytes per cell).  *rounds (may be NULL) receives how many
+ * rounds the chunked resolve took to settle.  It SYNCHRONIZES with `s` once per round.
+ * xrs_nb_jenks: the reference's _run_numpy_jenks_matrices over the n sorted float32 DEVICE values x for k classes:
+ * lower_class_limits to lcl (DEVICE float32, (k + 1) x (n + 1), column j at j (n + 1)) and var_combinations, laid
+ * out the same way, at the start of scratch (DEVICE, xrs_nb_jenks_scratch_bytes(n, k) bytes), bit for bit.
+ * (k - 1) n^2 / 2 iterations on top of the first column's n^2 / 2.  Enqueue-only.
+ * A bad argument returns XRS_EINVAL before any CUDA call. */
+int xrs_nb_sample_scratch_bytes(int64_t n, int64_t s, int64_t *bytes);
+int xrs_nb_sample(int64_t n, int64_t s, uint32_t seed, int64_t *out, void *scratch, int64_t scratch_bytes,
+                  int64_t *rounds, xrs_stream_t stream);
+int xrs_nb_jenks_scratch_bytes(int64_t n, int k, int64_t *bytes);
+int xrs_nb_jenks(const float *x, int64_t n, int k, float *lcl, void *scratch, int64_t scratch_bytes,
+                 xrs_stream_t stream);
+
 /* ------------------------------------------------------------------ host-buffer (end-to-end)
  * Same operators on HOST rasters: the library cuts the raster into row chunks and overlaps
  * host->device copies, kernels and device->host copies on internal streams.  `op` selects

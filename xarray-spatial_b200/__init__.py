@@ -8,7 +8,7 @@ from ._xr import DataArray, Dataset  # noqa: F401
 from .analytics import summarize_terrain, surface_suite  # noqa: F401
 from .aspect import aspect  # noqa: F401
 from .classify import binary, box_plot, equal_interval, head_tail_breaks, maximum_breaks  # noqa: F401
-from .classify import percentiles, quantile, reclassify, std_mean  # noqa: F401
+from .classify import natural_breaks, percentiles, quantile, reclassify, std_mean  # noqa: F401
 from .convolution import convolution_2d, convolve_2d  # noqa: F401
 from .curvature import curvature  # noqa: F401
 from .focal import apply as focal_apply  # noqa: F401

@@ -78,6 +78,10 @@ def _declare(lib):
         "xrs_classify_sort_scratch_bytes": [I64, I, ctypes.POINTER(I64)],
         "xrs_classify_sort": [P, I, I64, I64, I64, P, ctypes.POINTER(I64), P, I64, P],
         "xrs_classify_pick": [P, I, I64, I, ctypes.c_uint64, I64, P, I64, ctypes.POINTER(I64), P, P],
+        "xrs_nb_sample_scratch_bytes": [I64, I64, ctypes.POINTER(I64)],
+        "xrs_nb_sample": [I64, I64, ctypes.c_uint32, P, P, I64, ctypes.POINTER(I64), P],
+        "xrs_nb_jenks_scratch_bytes": [I64, I, ctypes.POINTER(I64)],
+        "xrs_nb_jenks": [P, I64, I, P, P, I64, P],
         "xrs_host_stencil":[I, P, I, P, I64, I64, P, P, I, P, I],
         "xrs_host_release": [I],
         "xrs_host_alloc": [ctypes.POINTER(P), I64],

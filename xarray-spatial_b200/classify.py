@@ -1,14 +1,19 @@
-"""binary, reclassify, quantile, percentiles, box_plot, equal_interval, std_mean, head_tail_breaks and
-maximum_breaks (classify.py of the reference) on the GPU, following the reference's NumPy path.
+"""binary, reclassify, quantile, percentiles, box_plot, equal_interval, std_mean, head_tail_breaks,
+maximum_breaks and natural_breaks (classify.py of the reference) on the GPU, following the reference's NumPy path.
 
 Every scheme ends in one per-cell pass: the reference's binary-search bin lookup (`_cpu_bin`) or the membership
 test of `binary` (`_cpu_binary`).  The breaks come from device work on the raster -- exact order statistics
 (radix select), one moments pass per level, or a radix sort -- and from the reference's own host arithmetic on
 the few scalars that work returns, restated line for line, so that they are NumPy's breaks bit for bit.  std_mean
 and head_tail_breaks take their means and deviations from float64 sums instead of NumPy's float32 pairwise ones
-(DESIGN.md section 4.11).  `natural_breaks` is not provided.
+(DESIGN.md section 4.11).
+
+natural_breaks draws the reference's seeded sample of cell indices on the device (RandomState(1234567890)'s shuffle,
+without the shuffle: xrs_nb_sample), sorts the sampled cells there, fills its Jenks matrices column by column on
+the device, bit for bit, and runs the reference's backtrack over them on the host.
 """
 import ctypes
+import warnings
 
 import numpy as np
 
@@ -147,6 +152,19 @@ class _Raster:
         self.call("xrs_classify_sort", self._ptr(), self.code, self._pitch(), H, W, ctypes.c_void_p(keys.data_ptr()),
                   ctypes.byref(n), ctypes.c_void_p(scratch.data_ptr()), size)
         return keys, n.value
+
+    def with_cells(self, t):
+        """The same cell type over other device cells `t` (2-D)."""
+        other = object.__new__(_Raster)
+        other.__dict__.update(self.__dict__)
+        other.t, other._hist0, other._n = t, None, None
+        return other
+
+    def sorted_values(self):
+        """The finite cells, sorted, on the host in the cells' own type: what the reference's data.sort() gives."""
+        keys, n = self.sorted_keys()
+        host = keys[:n].cpu().numpy().view(_key_dtype(self.cells))
+        return _values(host, self.cells).astype(self.dtype)
 
     def max_break_stats(self):
         gaps = _SortedGaps(self)
@@ -401,6 +419,114 @@ def maximum_breaks_bins(gaps, k):
     return np.append(bins, float(gaps.largest()))
 
 
+NB_SEED = 1234567890     # the reference's RandomState seed for natural_breaks' sample
+
+
+def _warn(message):
+    with warnings.catch_warnings():
+        warnings.simplefilter('default')
+        warnings.warn(message, Warning, stacklevel=4)
+
+
+def sample_indices(n, s, device, seed=NB_SEED):
+    """np.sort(idx[:s]) for idx = np.linspace(0, n, n, dtype=uint32) after RandomState(seed).shuffle(idx), on the
+    device as int64 (1 <= s < n <= 2^32)."""
+    import torch
+    need = ctypes.c_int64()
+    _lib.call("xrs_nb_sample_scratch_bytes", n, s, ctypes.byref(need))
+    scratch = torch.empty(need.value, dtype=torch.uint8, device=device)
+    out = torch.empty(s, dtype=torch.int64, device=device)
+    rounds = ctypes.c_int64()
+    with torch.cuda.device(device):
+        _lib.call("xrs_nb_sample", n, s, ctypes.c_uint32(seed), ctypes.c_void_p(out.data_ptr()),
+                  ctypes.c_void_p(scratch.data_ptr()), need.value, ctypes.byref(rounds),
+                  ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream))
+    return out
+
+
+def jenks_matrices(x, k):
+    """_run_numpy_jenks_matrices over the sorted float32 DEVICE values x: (lower_class_limits, var_combinations)
+    as DEVICE float32 tensors of shape (k + 1, n + 1), the transpose of the reference's."""
+    import torch
+    n = x.numel()
+    need = ctypes.c_int64()
+    _lib.call("xrs_nb_jenks_scratch_bytes", n, k, ctypes.byref(need))
+    scratch = torch.empty(need.value // 4, dtype=torch.float32, device=x.device)
+    lcl = torch.empty((k + 1, n + 1), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.call("xrs_nb_jenks", ctypes.c_void_p(x.data_ptr()), n, k, ctypes.c_void_p(lcl.data_ptr()),
+                  ctypes.c_void_p(scratch.data_ptr()), need.value,
+                  ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream))
+    return lcl, scratch[:(k + 1) * (n + 1)].view(k + 1, n + 1)
+
+
+def jenks_backtrack(data, lower_class_limits, n_classes, max_data):
+    """classify.py `_run_jenks` after the matrices, and `bins = centroids[1:]; bins[-1] = max_data`: data is the
+    sorted sample, lower_class_limits the (n + 1) x (k + 1) matrix."""
+    k = data.shape[0]
+    kclass = np.zeros(n_classes + 1, dtype=np.float32)
+    kclass[0] = data[0]
+    kclass[-1] = data[-1]
+    count_num = n_classes
+    while count_num > 1:
+        elt = int(lower_class_limits[k][count_num] - 2)
+        kclass[count_num - 1] = data[elt]
+        k = int(lower_class_limits[k][count_num] - 1)
+        count_num -= 1
+    bins = np.array(kclass[1:])
+    bins[-1] = max_data
+    return bins
+
+
+def natural_breaks_bins(r, num_sample, k):
+    """classify.py:589-664 `_compute_natural_break_bins` with `max_data` (classify.py:737-743): (bins, uvk)."""
+    n_finite, _, _, _, mx = r.moments()
+    if n_finite == 0:
+        np.max(np.empty(0, r.dtype))   # raises as the reference does
+    max_data = float(mx)
+    H, W = r.t.shape
+    num_data = H * W
+    sample = r
+    size = num_data
+    if num_sample is not None and num_sample < num_data:
+        size = len(range(num_data)[:num_sample])   # idx[:num_sample]: negative sizes count from the end
+        if size > 0:
+            idx = sample_indices(num_data, size, r.t.device)
+            # torch gathers unsigned 16- to 64-bit cells only through their signed view of the same width
+            signed = {r.torch.uint16: r.torch.int16, r.torch.uint32: r.torch.int32, r.torch.uint64: r.torch.int64}
+            t = r.t.view(signed[r.t.dtype]) if r.t.dtype in signed else r.t
+            sample = r.with_cells(t[idx // W, idx % W].view(r.t.dtype).view(1, size))
+        else:
+            sample = r.with_cells(r.t.new_empty((1, 0)))
+    if size >= 40000:
+        _warn('natural_breaks Warning: Natural break '
+              'classification (Jenks) has a complexity of O(n^2), '
+              'your classification with {} data points may take '
+              'a long time.'.format(size))
+    data = sample.sorted_values()
+    uvk = int(np.count_nonzero(data[1:] != data[:-1])) + 1 if data.size else 0
+    if uvk < k:
+        _warn('natural_breaks Warning: Not enough unique values '
+              'in data array for {} classes. '
+              'n_samples={} should be >= n_clusters={}. '
+              'Using k={} instead.'.format(k, uvk, k, uvk))
+        keep = np.ones(data.size, bool)
+        keep[1:] = data[1:] != data[:-1]
+        return data[keep], uvk
+    if not isinstance(k, (int, np.integer)):
+        raise TypeError("natural_breaks: k must be an integer, not {!r}".format(k))   # numba's typing error there
+    if k < -1:
+        raise ValueError("negative dimensions not allowed")   # np.zeros((n + 1, k + 1)) in the matrices
+    if k < 1:
+        raise IndexError("index -1 is out of bounds for axis 0 with size 0")   # kclass is too short
+    lcl = np.zeros((data.size + 1, k + 1), np.float32)
+    if k > 1:
+        import torch
+        x = torch.as_tensor(data.astype(np.float32), device=r.t.device)
+        lcl = jenks_matrices(x, k)[0].cpu().numpy().T
+    return jenks_backtrack(data, lcl, k, max_data), uvk
+
+
 # ---------------------------------------------------------------------- public functions
 def _bin(r, bins, new_values):
     return r.cells_pass(False, bins, new_values)
@@ -505,3 +631,13 @@ def maximum_breaks(agg, k=5, name='maximum_breaks'):
     r = _Raster(agg)
     bins = maximum_breaks_bins(r.max_break_stats(), k)
     return _wrap(_bin(r, bins, np.arange(len(bins))), r, agg, name)
+
+
+@supports_dataset
+def natural_breaks(agg, num_sample=20000, name='natural_breaks', k=5):
+    """Jenks natural breaks: the k classes of least within-class variance of a seeded sample of `num_sample` cells
+    (every cell when None or not less than the cell count), bounded above by the finite maximum
+    (classify.py:737-834).  The sample is the reference's; rasters of more than 2^32 cells raise ValueError."""
+    r = _Raster(agg)
+    bins, uvk = natural_breaks_bins(r, num_sample, k)
+    return _wrap(_bin(r, bins, np.arange(uvk)), r, agg, name)

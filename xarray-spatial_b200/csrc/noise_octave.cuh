@@ -1,7 +1,8 @@
 // noise_octave.cuh -- the exact arithmetic of perlin (perlin.py:189) and generate_terrain (terrain.py:183): NumPy's
-// legacy permutation (MT19937 and its masked-rejection draw), the reservation rule of the parallel Knuth shuffle,
-// and one octave of the reference's NumPy noise.  Everything here is __host__ __device__ and free of CUDA calls, so
-// the CPU tests compile this header with g++ and run the same steps as the kernels (noise.cu).
+// legacy permutation (MT19937 and its masked-rejection draw, from mt19937.cuh), the reservation rule of the
+// parallel Knuth shuffle, and one octave of the reference's NumPy noise.  Everything here is __host__ __device__
+// and free of CUDA calls, so the CPU tests compile this header with g++ and run the same steps as the kernels
+// (noise.cu).
 //
 // RandomState(seed).permutation(n) is init_genrand(seed), then Fisher-Yates from i = n - 1 down to 1: step i draws
 // tempered MT19937 words w until (w & mask(i)) <= i, mask(i) being i with every lower bit set, and swaps
@@ -10,76 +11,16 @@
 #include <math.h>
 #include <stdint.h>
 
-#ifndef __CUDACC__
-#define __host__
-#define __device__
-#endif
+#include "mt19937.cuh"
 
 namespace xrs {
 namespace nz {
 
-constexpr int kMtN = 624, kMtM = 397;
-constexpr uint32_t kMatrixA = 0x9908b0dfu, kUpper = 0x80000000u, kLower = 0x7fffffffu;
-// The twist of one 624-word block in four phases.  A word of one phase reads only words of earlier phases (new
-// values) or of later phases (old values), so each phase is parallel once all its reads precede its writes.
-// Phase p covers words [phase_begin(p), phase_begin(p + 1)): 0-226, 227-453, 454-622, 623.
-__host__ __device__ inline int phase_begin(int p) {
-    return p == 0 ? 0 : p == 1 ? kMtN - kMtM : p == 2 ? 2 * (kMtN - kMtM) : p == 3 ? kMtN - 1 : kMtN;
-}
+using namespace mt;   // the generator and the masked-rejection draw
 
 constexpr int64_t kTableN = (int64_t)1 << 20;   // the reference's table: permutation(2**20)
 constexpr int64_t kIndexLimit = 2 * kTableN;    // np.append(p, p) takes indices in [-2^21, 2^21)
 constexpr int kTerrainOctaves = 16;
-
-// init_genrand: NumPy's mt19937_seed for a seed in [0, 2^32 - 1].
-__host__ __device__ inline void mt_init(uint32_t *mt, uint32_t seed) {
-    mt[0] = seed;
-    for (int i = 1; i < kMtN; ++i) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (uint32_t)i;
-}
-
-// Word k of the next block, from the state as it stands.
-__host__ __device__ inline uint32_t mt_twist_word(const uint32_t *mt, int k) {
-    const uint32_t y = (mt[k] & kUpper) | (mt[k + 1 == kMtN ? 0 : k + 1] & kLower);
-    return mt[k + kMtM < kMtN ? k + kMtM : k + kMtM - kMtN] ^ (y >> 1) ^ ((0u - (y & 1u)) & kMatrixA);
-}
-
-__host__ __device__ inline void mt_twist(uint32_t *mt) {
-    for (int k = 0; k < kMtN; ++k) mt[k] = mt_twist_word(mt, k);
-}
-
-__host__ __device__ inline uint32_t mt_temper(uint32_t y) {
-    y ^= y >> 11;
-    y ^= (y << 7) & 0x9d2c5680u;
-    y ^= (y << 15) & 0xefc60000u;
-    return y ^ (y >> 18);
-}
-
-// random_interval's mask: the least 2^k - 1 >= i.
-__host__ __device__ inline uint32_t interval_mask(uint32_t i) {
-    i |= i >> 1;
-    i |= i >> 2;
-    i |= i >> 4;
-    i |= i >> 8;
-    return i | (i >> 16);
-}
-
-// One word of the sequential draw at step i (> 0): accepted when its masked value is at most i; then J[i] is that
-// value and the next step is i - 1.
-__host__ __device__ inline bool draw(uint32_t &i, uint32_t w, int32_t *J) {
-    const uint32_t v = w & interval_mask(i);
-    if (v > i) return false;
-    J[i] = (int32_t)v;
-    --i;
-    return true;
-}
-
-// The chunk rule of the warp resolve: 32 consecutive words meet steps i, i - 1, ..., i - 31 at most.  When every
-// step of that range has the same mask and i >= 32, a word whose masked value is at most i - 31 is accepted
-// whatever the words before it did, and one above i is rejected.  Only words in between depend on their
-// predecessors; a chunk holding one, or not uniform, is resolved word by word.
-__host__ __device__ inline bool chunk_uniform(uint32_t i) { return i >= 32 && interval_mask(i - 31) == interval_mask(i); }
-__host__ __device__ inline bool sure_accept(uint32_t v, uint32_t i) { return v <= i - 31; }
-__host__ __device__ inline bool undecided(uint32_t v, uint32_t i) { return v > i - 31 && v <= i; }
 
 // The deterministic reservations of the parallel Knuth shuffle (Shun, Gu, Blelloch, Fineman and Gibbons, SODA
 // 2015): in round r every pending step i writes max(key) to positions i and J[i], and commits its swap when it
