@@ -48,8 +48,9 @@ enum xrs_focal_stat {
     XRS_STAT_STD = 4, XRS_STAT_RANGE = 5, XRS_STAT_VAR = 6
 };
 
-/* element types for zonal inputs */
-enum xrs_dtype { XRS_F32 = 0, XRS_F64 = 1, XRS_I32 = 2, XRS_I64 = 3, XRS_I16 = 4, XRS_U16 = 5 };
+/* element types for zonal inputs; 6-10 are read only by xrs_zonal_regions and xrs_zonal_bounds */
+enum xrs_dtype { XRS_F32 = 0, XRS_F64 = 1, XRS_I32 = 2, XRS_I64 = 3, XRS_I16 = 4, XRS_U16 = 5,
+                 XRS_I8 = 6, XRS_U8 = 7, XRS_U32 = 8, XRS_U64 = 9, XRS_BOOL = 10 };
 
 int xrs_abi_version(void);
 const char *xrs_last_error_string(void);
@@ -376,6 +377,26 @@ int xrs_nb_sample(int64_t n, int64_t s, uint32_t seed, int64_t *out, void *scrat
 int xrs_nb_jenks_scratch_bytes(int64_t n, int k, int64_t *bytes);
 int xrs_nb_jenks(const float *x, int64_t n, int k, float *lcl, void *scratch, int64_t scratch_bytes,
                  xrs_stream_t stream);
+
+/* ------------------------------------------------------------------ zonal regions / trim / crop (zonal_regions.cu)
+ * Rasters of H x W cells of `dtype` (any xrs_dtype), rows in_pitch bytes apart, H and W below 2^31, read and never
+ * written.
+ * xrs_zonal_regions: zonal.regions (zonal.py:1406-1549): the reference's label of every cell for the 4- or 8-cell
+ * neighbourhood, as int64 cast once to the cell type (bool: all true), NaN for NaN cells, to out (DEVICE, the cell
+ * type, rows out_pitch bytes apart).  scratch: a DEVICE buffer of at least xrs_zonal_regions_scratch_bytes(H, W)
+ * bytes (10 bytes per cell below 2^31 cells, 18 above).  Enqueue-only.
+ * xrs_zonal_bounds: the least and largest row, then the least and largest column, of the cells that equal none of
+ * the n_values values (mode 0, zonal.trim) or one of them (mode 1, zonal.crop), as int64 to out4 (DEVICE); rows
+ * LLONG_MAX, -1 and columns LLONG_MAX, -1 when no cell qualifies.  values (DEVICE float64) holds the values;
+ * int_values (DEVICE int64, or NULL when any value is not an integer) holds them again as integers, and integer
+ * cells other than uint64 then compare exactly; everything else compares in float64, where NaN equals nothing.
+ * Enqueue-only.
+ * A bad argument returns XRS_EINVAL before any CUDA call. */
+int xrs_zonal_regions_scratch_bytes(int64_t H, int64_t W, int64_t *bytes);
+int xrs_zonal_regions(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W, int neighborhood, void *out,
+                      int64_t out_pitch, void *scratch, int64_t scratch_bytes, xrs_stream_t s);
+int xrs_zonal_bounds(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W, int mode,
+                     const double *values, const int64_t *int_values, int n_values, int64_t *out4, xrs_stream_t s);
 
 /* ------------------------------------------------------------------ host-buffer (end-to-end)
  * Same operators on HOST rasters: the library cuts the raster into row chunks and overlaps

@@ -22,6 +22,7 @@ from .multispectral import arvi, ebbi, evi, gci, nbr, nbr2, ndmi, ndvi, savi, si
 from .slope import slope  # noqa: F401
 from .terrain import generate_terrain  # noqa: F401
 from .viewshed import viewshed  # noqa: F401
+from .zonal import crop, regions, suggest_zonal_canvas, trim  # noqa: F401
 from .zonal import crosstab as zonal_crosstab  # noqa: F401
 from .zonal import stats as zonal_stats  # noqa: F401
 

@@ -13,6 +13,8 @@ XRS_OK, XRS_EINVAL, XRS_ECUDA, XRS_EUNSUPPORTED, XRS_ENOMEM = 0, -1, -2, -3, -4
 OPS = dict(slope=0, aspect=1, curvature=2, hillshade=3, focal_mean=4, convolve=5, focal_stat=6)
 STATS = dict(mean=0, sum=1, min=2, max=3, std=4, range=5, var=6)
 DTYPES = dict(float32=0, float64=1, int32=2, int64=3, int16=4, uint16=5)
+# every cell type xrs_zonal_regions and xrs_zonal_bounds read as they are
+ZONAL_CELLS = dict(DTYPES, int8=6, uint8=7, uint32=8, uint64=9, bool=10)
 
 _lib = None
 
@@ -82,6 +84,9 @@ def _declare(lib):
         "xrs_nb_sample": [I64, I64, ctypes.c_uint32, P, P, I64, ctypes.POINTER(I64), P],
         "xrs_nb_jenks_scratch_bytes": [I64, I, ctypes.POINTER(I64)],
         "xrs_nb_jenks": [P, I64, I, P, P, I64, P],
+        "xrs_zonal_regions_scratch_bytes": [I64, I64, ctypes.POINTER(I64)],
+        "xrs_zonal_regions": [P, I, I64, I64, I64, I, P, I64, P, I64, P],
+        "xrs_zonal_bounds": [P, I, I64, I64, I64, I, P, P, I, P, P],
         "xrs_host_stencil":[I, P, I, P, I64, I64, P, P, I, P, I],
         "xrs_host_release": [I],
         "xrs_host_alloc": [ctypes.POINTER(P), I64],

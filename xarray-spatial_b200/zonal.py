@@ -9,14 +9,15 @@ by one sort.  With `comm` (a torch.distributed process group) the partials of ro
 are combined with AllReduce before finalisation.
 """
 import ctypes
+import math
 
 import numpy as np
 import pandas as pd
 
 from . import _lib
 from ._xr import DataArray, Dataset
-from .utils import (ArrayTypeFunctionMapping, as_device_tensor, like_container, stream_ptr,
-                    validate_arrays)
+from .utils import (ArrayTypeFunctionMapping, as_device_tensor, is_dask_array, is_device_array, like_container,
+                    stream_ptr, validate_arrays)
 
 _DEFAULT_STATS = ("mean", "max", "min", "sum", "std", "var", "count", "majority")
 
@@ -800,3 +801,139 @@ def crosstab(zones, values, zone_ids=None, cat_ids=None, layer=None, agg="count"
         for c in cats:
             d[c] = table[c]
     return pd.DataFrame(d)
+
+
+# ----------------------------------------------------------------------------- regions, trim, crop
+def _raster_cells(data, what):
+    """The raster as a 2-D CUDA tensor with unit column stride, and its cell type's code for zonal_regions.cu."""
+    import torch
+    if is_dask_array(data):
+        raise NotImplementedError("%s: Dask arrays are not supported by the GPU backend" % what)
+    if isinstance(data, np.ndarray):
+        if data.dtype == np.float16:
+            raise NotImplementedError("%s: float16 rasters are not supported (nor by the reference)" % what)
+        t = torch.from_numpy(np.ascontiguousarray(data)).cuda()
+    elif is_device_array(data):
+        t = as_device_tensor(data)
+    else:
+        raise TypeError("Unsupported raster array type: {}".format(type(data)))
+    if t.ndim != 2:
+        raise ValueError("%s needs a 2-D raster, got %d dimensions" % (what, t.ndim))
+    code = _lib.ZONAL_CELLS.get(str(t.dtype).replace("torch.", ""))
+    if code is None:
+        raise NotImplementedError("%s: %s rasters are not supported (nor by the reference)" % (what, t.dtype))
+    if t.stride(1) != 1 or t.stride(0) < t.shape[1]:
+        t = t.contiguous()
+    return t, code
+
+
+def _pitch(t):
+    return max(t.stride(0), t.shape[1]) * t.element_size()
+
+
+def regions(raster, neighborhood=4, name="regions"):
+    """Number the connected regions of cells with close values (zonal.py:1552-1640 of the reference).
+
+    Cells join their 4 or 8 neighbours when |neighbour - cell| <= 1e-08 + 1e-05 |cell|, evaluated as the
+    reference's numba kernel evaluates it for the cell type.  Every cell gets the label the reference's two-pass
+    scan gives it, in the raster's cell type (labels are not renumbered, so they may have gaps); NaN cells stay
+    NaN, and a bool raster gives all True.  Labels are exact in int64 before the one cast to the cell type, where
+    the reference's own labels wrap or round once they pass the type's range (DESIGN.md section 4.12)."""
+    import torch
+    if neighborhood not in (4, 8):
+        raise ValueError("`neighborhood` value must be either 4 or 8)")
+    data = raster.data
+    t, code = _raster_cells(data, "regions")
+    H, W = t.shape
+    out = torch.empty((H, W), dtype=t.dtype, device=t.device)
+    if H and W:
+        need = ctypes.c_int64()
+        _lib.call("xrs_zonal_regions_scratch_bytes", H, W, ctypes.byref(need))
+        try:
+            scratch = torch.empty(need.value, dtype=torch.uint8, device=t.device)
+        except torch.OutOfMemoryError as e:
+            raise MemoryError("regions needs %d bytes of device scratch for a %d x %d raster"
+                              % (need.value, H, W)) from e
+        with torch.cuda.device(t.device):
+            _lib.call("xrs_zonal_regions", _ptr(t), code, _pitch(t), H, W, neighborhood, _ptr(out),
+                      W * out.element_size(), _ptr(scratch), need.value, stream_ptr(t))
+    result = out.cpu().numpy() if isinstance(data, np.ndarray) else like_container(out, data)
+    return DataArray(result, name=name, dims=raster.dims, coords=raster.coords, attrs=raster.attrs)
+
+
+def _bounds(data, values, mode, what):
+    """(top, bottom, left, right) as the reference's _trim (mode 0) or _crop (mode 1) finds them: the first and
+    last rows and columns holding a cell that equals none of `values` (trim) or one of them (crop), and
+    (rows - 1, 0, cols - 1, 0) when no cell does."""
+    import torch
+    t, code = _raster_cells(data, what)
+    H, W = t.shape
+    vals = list(values)
+    # numba types a list of ints as int64 and compares integer cells with them exactly; any float makes it float64
+    ints = all(isinstance(v, (int, np.integer, np.bool_)) for v in vals)
+    dv = torch.tensor([float(v) for v in vals], dtype=torch.float64, device=t.device)
+    iv = torch.tensor([int(v) for v in vals], dtype=torch.int64, device=t.device) if ints and vals else None
+    out4 = torch.empty(4, dtype=torch.int64, device=t.device)
+    with torch.cuda.device(t.device):
+        _lib.call("xrs_zonal_bounds", _ptr(t), code, _pitch(t), H, W, mode, _ptr(dv) if vals else None,
+                  _ptr(iv) if iv is not None else None, len(vals), _ptr(out4), stream_ptr(t))
+    top, bottom, left, right = out4.cpu().tolist()
+    if bottom < 0:
+        return max(H - 1, 0), 0, max(W - 1, 0), 0
+    return top, bottom, left, right
+
+
+def _window(raster, top, bottom, left, right, name):
+    """raster[top:bottom + 1, left:right + 1] with its coordinates sliced alike (the shim DataArray has no
+    positional indexing)."""
+    rs, cs = slice(top, bottom + 1), slice(left, right + 1)
+    by_dim = dict(zip(raster.dims, (rs, cs)))
+    coords = {}
+    for k, v in raster.coords.items():
+        dims = getattr(v, "dims", None)
+        v = v.data if dims is not None else v
+        shape = tuple(getattr(v, "shape", ()))
+        if dims is None:   # shim coordinates are bare arrays: a 1-D one named after a dimension runs along it
+            dims = (k,) if len(shape) == 1 and k in by_dim else tuple(raster.dims) if shape == raster.shape else ()
+        if len(dims) == len(shape) and any(d in by_dim for d in dims):
+            v = DataArray(v[tuple(by_dim.get(d, slice(None)) for d in dims)], dims=dims)
+        coords[k] = v
+    return DataArray(raster.data[rs, cs], name=name, dims=raster.dims, coords=coords, attrs=raster.attrs)
+
+
+def trim(raster, values=(np.nan,), name="trim"):
+    """Drop the edge rows and columns that hold only `values` (zonal.py:1734-1842 of the reference).
+
+    Cells equal a value as in the reference's numba loop: integer cells and integer values exactly, anything
+    with a float in float64, NaN never (so the default trims nothing).  When every cell is one of the values the
+    reference's bounds (rows - 1, 0, cols - 1, 0) give an empty result unless that side has length 1."""
+    top, bottom, left, right = _bounds(raster.data, values, 0, "trim")
+    return _window(raster, top, bottom, left, right, name)
+
+
+def crop(zones, values, zones_ids, name="crop"):
+    """Cut `values` to the rows and columns between the first and last cells of `zones` equal to one of
+    `zones_ids` (zonal.py:1943-2062 of the reference); equality as in trim."""
+    top, bottom, left, right = _bounds(zones.data, zones_ids, 1, "crop")
+    return _window(values, top, bottom, left, right, name)
+
+
+# ----------------------------------------------------------------------------- canvas size
+_FULL_EXTENTS = {"Mercator": ((-20e6, 20e6), (-20e6, 20e6)), "Geographic": ((-180, 180), (-90, 90))}
+
+
+def get_full_extent(crs):
+    """((min_x, max_x), (min_y, max_y)) of the 'Mercator' or 'Geographic' projection; KeyError for others."""
+    return _FULL_EXTENTS[crs]
+
+
+def suggest_zonal_canvas(smallest_area, x_range, y_range, crs="Mercator", min_pixels=25):
+    """(height, width) of a canvas over x_range x y_range on which a polygon of `smallest_area` covers about
+    `min_pixels` pixels, with the pixels as square as the projection's full extent allows (zonal.py:1304-1403
+    of the reference, in its float operations)."""
+    (x0, x1), (y0, y1) = get_full_extent(crs)
+    aspect = (x1 - x0) / (y1 - y0)
+    pixels = (x1 - x0) * (y1 - y0) / (smallest_area / min_pixels)
+    h = math.sqrt(pixels / aspect)
+    w = aspect * h
+    return int(h * (y_range[1] - y_range[0]) / (y1 - y0)), int(w * (x_range[1] - x_range[0]) / (x1 - x0))
