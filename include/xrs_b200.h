@@ -48,7 +48,11 @@ enum xrs_focal_stat {
     XRS_STAT_STD = 4, XRS_STAT_RANGE = 5, XRS_STAT_VAR = 6
 };
 
-/* element types for zonal inputs; 6-10 are read only by xrs_zonal_regions and xrs_zonal_bounds */
+/* cell types of raster arguments.  Two sets of them:
+ *   the raster set, XRS_F32 .. XRS_U16 (codes 0-5): read by proximity, viewshed, a_star_search and classify;
+ *   the zonal set, every code (0-10): read by xrs_zonal_regions and xrs_zonal_bounds.
+ * A code outside an entry point's set returns XRS_EINVAL ("unknown cell type"); its input pitch must be a multiple
+ * of the cell size and at least a row. */
 enum xrs_dtype { XRS_F32 = 0, XRS_F64 = 1, XRS_I32 = 2, XRS_I64 = 3, XRS_I16 = 4, XRS_U16 = 5,
                  XRS_I8 = 6, XRS_U8 = 7, XRS_U32 = 8, XRS_U64 = 9, XRS_BOOL = 10 };
 
@@ -234,8 +238,8 @@ int xrs_zonal_pair_count(const float *values, const int32_t *zones, int64_t n, i
 /* ------------------------------------------------------------------ proximity
  * proximity / allocation / direction (proximity.py:401-647) as an exact nearest-target transform: every cell gets
  * the target nearest to it under the metric, the first in row-major order among equidistant ones (the reference's
- * GDAL-style sweep only approximates this; DESIGN.md section 4.7).  Rasters of H x W cells of in_dtype (any
- * xrs_dtype), rows in_pitch bytes apart; x[W] and y[H] are DEVICE float64 coordinates, each strictly ascending
+ * GDAL-style sweep only approximates this; DESIGN.md section 4.7).  Rasters of H x W cells of in_dtype (the raster
+ * set), rows in_pitch bytes apart; x[W] and y[H] are DEVICE float64 coordinates, each strictly ascending
  * or strictly descending (GREAT_CIRCLE: degrees of longitude / latitude within +-180 / +-90).
  * targets: NULL for the default rule (nonzero and finite cells), else a DEVICE array of n_targets float64
  * values sorted ascending without NaN (a cell is a target when its value, widened to float64, is one of them;
@@ -256,8 +260,8 @@ int xrs_proximity(const void *in, int in_dtype, int64_t in_pitch, int64_t H, int
 
 /* ------------------------------------------------------------------ viewshed
  * viewshed (viewshed.py:1122-1502) as a per-cell line-of-sight test that makes the reference sweep's
- * visible / invisible decision (DESIGN.md section 4.8).  Rasters of H x W cells of in_dtype (any xrs_dtype, read
- * as float64, never written), rows in_pitch bytes apart; the observer stands on cell (vp_row, vp_col) at
+ * visible / invisible decision (DESIGN.md section 4.8).  Rasters of H x W cells of in_dtype (the raster set,
+ * read as float64, never written), rows in_pitch bytes apart; the observer stands on cell (vp_row, vp_col) at
  * vp_elev; target_elev is added to every cell seen as a target; ew_res / ns_res are the coordinate steps between
  * columns / rows (may be negative or NaN).  float64 output, rows out_pitch bytes apart: 180 at the observer, the
  * vertical angle in degrees of a visible cell, -1 otherwise (NaN cells never block and are -1).
@@ -270,7 +274,7 @@ int xrs_viewshed(const void *in, int in_dtype, int64_t in_pitch, int64_t H, int6
 
 /* ------------------------------------------------------------------ a_star_search
  * a_star_search (pathfinding.py:233-382) as an exact shortest-path search (DESIGN.md section 4.9).  Rasters of
- * H x W cells of in_dtype (any xrs_dtype, read as float64, never written), rows in_pitch bytes apart, H W < 2^31.
+ * H x W cells of in_dtype (the raster set, read as float64, never written), rows in_pitch bytes apart, H W < 2^31.
  * A cell is crossable unless it is NaN or equal to one of the n_barriers DEVICE float64 values in `barriers`
  * (NULL when n_barriers is 0).  Moves go to the 8 neighbours, or 4 with connectivity 4, and cost 1 or sqrt(2).
  * xrs_a_star_search: float64 output, rows out_pitch bytes apart, NaN except along a shortest path from the start
@@ -322,7 +326,7 @@ int xrs_noise(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W,
               int32_t *index_stats, void *scratch, int64_t scratch_bytes, xrs_stream_t s);
 
 /* ------------------------------------------------------------------ classify (classify.cu)
- * Rasters are H x W cells of `dtype` (any xrs_dtype), rows in_pitch bytes apart, read and never written.  A key is
+ * Rasters are H x W cells of `dtype` (the raster set), rows in_pitch bytes apart, read and never written.  A key is
  * the order-preserving unsigned image of a cell's bits (-0.0 folded into +0.0; 16-, 32- or 64-bit by the cell
  * type); "finite" is every integer cell and the float cells that are neither NaN nor +-inf.
  * xrs_classify_cells: member 0 is the reference's _cpu_bin: each finite cell is compared in float64 with bins[nb]
@@ -379,7 +383,7 @@ int xrs_nb_jenks(const float *x, int64_t n, int k, float *lcl, void *scratch, in
                  xrs_stream_t stream);
 
 /* ------------------------------------------------------------------ zonal regions / trim / crop (zonal_regions.cu)
- * Rasters of H x W cells of `dtype` (any xrs_dtype), rows in_pitch bytes apart, H and W below 2^31, read and never
+ * Rasters of H x W cells of `dtype` (the zonal set), rows in_pitch bytes apart, H and W below 2^31, read and never
  * written.
  * xrs_zonal_regions: zonal.regions (zonal.py:1406-1549): the reference's label of every cell for the 4- or 8-cell
  * neighbourhood, as int64 cast once to the cell type (bool: all true), NaN for NaN cells, to out (DEVICE, the cell

@@ -20,8 +20,7 @@ import numpy as np
 from . import _lib
 from ._xr import DataArray
 from .dataset_support import supports_dataset
-from .proximity import _cells
-from .utils import is_dask_array, is_device_array, like_container, stream_ptr
+from .utils import call_on, device_cells, device_scratch, pitch, ptr, to_container
 
 CELLS, GAPS, TIE_POSITIONS = 0, 1, 2    # key sources of xrs_classify_select
 _KEY_BITS = {np.dtype(np.float64): 64, np.dtype(np.int64): 64, np.dtype(np.int16): 16, np.dtype(np.uint16): 16}
@@ -51,12 +50,8 @@ class _Raster:
     def __init__(self, agg):
         import torch
         data = agg.data
-        if is_dask_array(data):
-            raise NotImplementedError("classify: Dask arrays are not supported by the GPU backend")
-        if not (isinstance(data, np.ndarray) or is_device_array(data)):
-            raise TypeError("Unsupported Array Type: {}".format(type(data)))
         self.data = data
-        self.t, self.code = _cells(data)
+        self.t, self.code = device_cells(data, "classify", "widen")
         self.cells = np.dtype(str(self.t.dtype).replace("torch.", ""))
         if isinstance(data, np.ndarray):
             self.dtype = data.dtype
@@ -65,21 +60,6 @@ class _Raster:
             self.dtype = np.dtype(src) if src not in ("bfloat16",) else self.cells
         self.torch = torch
         self._hist0 = self._n = None
-
-    def call(self, name, *args):
-        with self.torch.cuda.device(self.t.device):
-            _lib.call(name, *args, stream_ptr(self.t))
-
-    def _ptr(self):
-        return ctypes.c_void_p(self.t.data_ptr())
-
-    def _pitch(self):
-        return self.t.stride(0) * self.t.element_size() if self.t.dim() == 2 else 0
-
-    def scratch(self, query, *args):
-        need = ctypes.c_int64()
-        _lib.call(query, *args, ctypes.byref(need))
-        return self.torch.empty(max(1, need.value), dtype=self.torch.uint8, device=self.t.device), need.value
 
     # ------------------------------------------------------------------ device work
     def cells_pass(self, member, table, new_values=None):
@@ -97,47 +77,45 @@ class _Raster:
             nv = np.append(nv, np.full(nb + 1 - nv.size, np.nan, np.float32))
             dev_new = torch.as_tensor(nv, device=self.t.device)
         if H and W:
-            self.call("xrs_classify_cells", self._ptr(), self.code, self._pitch(), H, W, int(member),
-                      ctypes.c_void_p(dev_tab.data_ptr()),
-                      None if dev_new is None else ctypes.c_void_p(dev_new.data_ptr()), nb,
-                      ctypes.c_void_p(out.data_ptr()), out.stride(0) * out.element_size())
+            call_on(self.t, "xrs_classify_cells", ptr(self.t), self.code, pitch(self.t), H, W, int(member),
+                    ptr(dev_tab), None if dev_new is None else ptr(dev_new), nb, ptr(out), pitch(out))
         return out
 
     def moments(self, above=-np.inf):
         """(count, mean, M2, min, max) of the finite cells above `above`, in float64."""
         H, W = self.t.shape
-        scratch, size = self.scratch("xrs_classify_moments_scratch_bytes")
+        scratch, size = device_scratch("xrs_classify_moments_scratch_bytes", device=self.t.device, what="classify")
         out = self.torch.empty(5, dtype=self.torch.float64, device=self.t.device)
-        self.call("xrs_classify_moments", self._ptr(), self.code, self._pitch(), H, W, float(above),
-                  ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(scratch.data_ptr()), size)
+        call_on(self.t, "xrs_classify_moments", ptr(self.t), self.code, pitch(self.t), H, W, float(above), ptr(out),
+                ptr(scratch), size)
         n, mean, m2, mn, mx = out.cpu().numpy().tolist()
         return int(n), mean, m2, mn, mx
 
-    def _select(self, source, ptr, H, W, bits, ranks, hist0, tie=0):
-        scratch, size = self.scratch("xrs_classify_select_scratch_bytes")
+    def _select(self, source, keys_ptr, H, W, bits, ranks, hist0, tie=0):
+        scratch, size = device_scratch("xrs_classify_select_scratch_bytes", device=self.t.device, what="classify")
         ranks = np.ascontiguousarray(ranks, dtype=np.int64)
         nr = ranks.size
         keys = np.zeros(max(1, nr), np.uint64)
         rem = np.zeros(max(1, nr), np.int64)
         n = ctypes.c_int64()
-        self.call("xrs_classify_select", source, ptr, self.code, self._pitch() if source == CELLS else 0, H, W,
-                  bits, ctypes.c_uint64(tie), ranks.ctypes.data_as(ctypes.c_void_p), nr,
-                  keys.ctypes.data_as(ctypes.c_void_p), rem.ctypes.data_as(ctypes.c_void_p), ctypes.byref(n),
-                  hist0.ctypes.data_as(ctypes.c_void_p), ctypes.c_void_p(scratch.data_ptr()), size)
+        call_on(self.t, "xrs_classify_select", source, keys_ptr, self.code, pitch(self.t) if source == CELLS else 0, H,
+                W, bits, ctypes.c_uint64(tie), ranks.ctypes.data_as(ctypes.c_void_p), nr,
+                keys.ctypes.data_as(ctypes.c_void_p), rem.ctypes.data_as(ctypes.c_void_p), ctypes.byref(n),
+                hist0.ctypes.data_as(ctypes.c_void_p), ptr(scratch), size)
         return n.value, keys[:nr], rem[:nr]
 
     def finite_count(self):
         if self._n is None:
             self._hist0 = np.zeros(256, np.uint64)
             H, W = self.t.shape
-            self._n = self._select(CELLS, self._ptr(), H, W, _KEY_BITS.get(self.cells, 32), [], self._hist0)[0]
+            self._n = self._select(CELLS, ptr(self.t), H, W, _KEY_BITS.get(self.cells, 32), [], self._hist0)[0]
         return self._n
 
     def order_stats(self, ranks):
         """The finite cells at 0-based `ranks` of their ascending order, as `dtype`: one set of digit passes."""
         self.finite_count()
         H, W = self.t.shape
-        _, keys, _ = self._select(CELLS, self._ptr(), H, W, _KEY_BITS.get(self.cells, 32), ranks, self._hist0)
+        _, keys, _ = self._select(CELLS, ptr(self.t), H, W, _KEY_BITS.get(self.cells, 32), ranks, self._hist0)
         return _values(keys, self.cells).astype(self.dtype)
 
     def sorted_keys(self):
@@ -147,10 +125,11 @@ class _Raster:
         kt = _key_dtype(self.cells)
         keys = torch.empty(max(1, H * W), dtype=torch.int64 if kt == np.uint64 else torch.int32,
                            device=self.t.device)
-        scratch, size = self.scratch("xrs_classify_sort_scratch_bytes", H * W, self.code)
+        scratch, size = device_scratch("xrs_classify_sort_scratch_bytes", H * W, self.code, device=self.t.device,
+                                       what="classify")
         n = ctypes.c_int64()
-        self.call("xrs_classify_sort", self._ptr(), self.code, self._pitch(), H, W, ctypes.c_void_p(keys.data_ptr()),
-                  ctypes.byref(n), ctypes.c_void_p(scratch.data_ptr()), size)
+        call_on(self.t, "xrs_classify_sort", ptr(self.t), self.code, pitch(self.t), H, W, ptr(keys), ctypes.byref(n),
+                ptr(scratch), size)
         return keys, n.value
 
     def with_cells(self, t):
@@ -181,7 +160,7 @@ class _SortedGaps:
     def __init__(self, r):
         self.r = r
         self.keys, self.n = r.sorted_keys()
-        self.ptr = ctypes.c_void_p(self.keys.data_ptr())
+        self.ptr = ptr(self.keys)
         self.bits = _KEY_BITS.get(r.cells, 32)
         self.hist0 = np.zeros(256, np.uint64)
         self.n_gaps = r._select(GAPS, self.ptr, 1, self.n, self.bits, [], self.hist0)[0] if self.n else 0
@@ -197,8 +176,8 @@ class _SortedGaps:
         out = torch.empty(max(1, cap * (1 + mode)), dtype=self.keys.dtype, device=self.keys.device)
         scratch = torch.empty(8, dtype=torch.uint8, device=self.keys.device)
         count = ctypes.c_int64()
-        self.r.call("xrs_classify_pick", self.ptr, self.r.code, self.n, mode, ctypes.c_uint64(tie), pos,
-                    ctypes.c_void_p(out.data_ptr()), cap, ctypes.byref(count), ctypes.c_void_p(scratch.data_ptr()))
+        call_on(self.r.t, "xrs_classify_pick", self.ptr, self.r.code, self.n, mode, ctypes.c_uint64(tie), pos,
+                ptr(out), cap, ctypes.byref(count), ptr(scratch))
         if count.value != cap:
             raise _lib.XrsError("classify pick found %d entries, expected %d" % (count.value, cap))
         return self._host_keys(out[:cap * (1 + mode)])
@@ -432,15 +411,10 @@ def sample_indices(n, s, device, seed=NB_SEED):
     """np.sort(idx[:s]) for idx = np.linspace(0, n, n, dtype=uint32) after RandomState(seed).shuffle(idx), on the
     device as int64 (1 <= s < n <= 2^32)."""
     import torch
-    need = ctypes.c_int64()
-    _lib.call("xrs_nb_sample_scratch_bytes", n, s, ctypes.byref(need))
-    scratch = torch.empty(need.value, dtype=torch.uint8, device=device)
+    scratch, size = device_scratch("xrs_nb_sample_scratch_bytes", n, s, device=device, what="natural_breaks' sample")
     out = torch.empty(s, dtype=torch.int64, device=device)
     rounds = ctypes.c_int64()
-    with torch.cuda.device(device):
-        _lib.call("xrs_nb_sample", n, s, ctypes.c_uint32(seed), ctypes.c_void_p(out.data_ptr()),
-                  ctypes.c_void_p(scratch.data_ptr()), need.value, ctypes.byref(rounds),
-                  ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream))
+    call_on(out, "xrs_nb_sample", n, s, ctypes.c_uint32(seed), ptr(out), ptr(scratch), size, ctypes.byref(rounds))
     return out
 
 
@@ -449,15 +423,11 @@ def jenks_matrices(x, k):
     as DEVICE float32 tensors of shape (k + 1, n + 1), the transpose of the reference's."""
     import torch
     n = x.numel()
-    need = ctypes.c_int64()
-    _lib.call("xrs_nb_jenks_scratch_bytes", n, k, ctypes.byref(need))
-    scratch = torch.empty(need.value // 4, dtype=torch.float32, device=x.device)
+    scratch, size = device_scratch("xrs_nb_jenks_scratch_bytes", n, k, device=x.device,
+                                   what="natural_breaks' Jenks matrices")
     lcl = torch.empty((k + 1, n + 1), dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        _lib.call("xrs_nb_jenks", ctypes.c_void_p(x.data_ptr()), n, k, ctypes.c_void_p(lcl.data_ptr()),
-                  ctypes.c_void_p(scratch.data_ptr()), need.value,
-                  ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream))
-    return lcl, scratch[:(k + 1) * (n + 1)].view(k + 1, n + 1)
+    call_on(x, "xrs_nb_jenks", ptr(x), n, k, ptr(lcl), ptr(scratch), size)
+    return lcl, scratch.view(torch.float32)[:(k + 1) * (n + 1)].view(k + 1, n + 1)
 
 
 def jenks_backtrack(data, lower_class_limits, n_classes, max_data):
@@ -533,12 +503,8 @@ def _bin(r, bins, new_values):
 
 
 def _wrap(out, r, agg, name):
-    if isinstance(out, np.ndarray):
-        pass
-    elif isinstance(r.data, np.ndarray):
-        out = out.cpu().numpy()
-    else:
-        out = like_container(out, r.data)
+    if not isinstance(out, np.ndarray):
+        out = to_container(out, r.data)
     return DataArray(out, name=name, dims=agg.dims, coords=agg.coords, attrs=agg.attrs)
 
 

@@ -33,7 +33,7 @@ template <typename T> __device__ __forceinline__ uint64_t key_of(T v) {
         return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);
     } else if constexpr (std::is_same_v<T, int32_t>) {
         return (uint32_t)v ^ 0x80000000u;
-    } else if constexpr (std::is_same_v<T, int64_t>) {
+    } else if constexpr (std::is_same_v<T, long long>) {
         return (uint64_t)v ^ 0x8000000000000000ull;
     } else if constexpr (std::is_same_v<T, int16_t>) {
         return (uint16_t)v ^ 0x8000u;
@@ -51,8 +51,8 @@ template <typename T> __device__ __forceinline__ T value_of(uint64_t k) {
         return __longlong_as_double((long long)((k & 0x8000000000000000ull) ? (k & 0x7fffffffffffffffull) : ~k));
     } else if constexpr (std::is_same_v<T, int32_t>) {
         return (int32_t)((uint32_t)k ^ 0x80000000u);
-    } else if constexpr (std::is_same_v<T, int64_t>) {
-        return (int64_t)(k ^ 0x8000000000000000ull);
+    } else if constexpr (std::is_same_v<T, long long>) {
+        return (long long)(k ^ 0x8000000000000000ull);
     } else if constexpr (std::is_same_v<T, int16_t>) {
         return (int16_t)(uint16_t)((uint32_t)k ^ 0x8000u);
     } else {
@@ -615,18 +615,6 @@ int key_bits(int dtype) {
     }
 }
 
-template <typename F> int with_cell_type(int dtype, F &&f) {
-    switch (dtype) {
-        case XRS_F32: return f(float{});
-        case XRS_F64: return f(double{});
-        case XRS_I32: return f(int32_t{});
-        case XRS_I64: return f(int64_t{});
-        case XRS_I16: return f(int16_t{});
-        case XRS_U16: return f(uint16_t{});
-        default: set_error("unknown cell type %d", dtype); return XRS_EINVAL;
-    }
-}
-
 // The histogram of one digit pass over `src` for the sorted prefixes, copied to `host` (G x 256).
 template <typename Src>
 int select_pass(const Src &src, int64_t H, int64_t W, const std::vector<uint64_t> &prefixes, int lo,
@@ -718,8 +706,9 @@ int xrs_classify_cells(const void *in, int dtype, int64_t in_pitch, int64_t H, i
     XRS_REQUIRE(H >= 0 && W >= 0 && nb >= 0, "bad shape");
     if (H == 0 || W == 0) return XRS_OK;
     XRS_REQUIRE(in && out && (nb == 0 || (bins && (member || new_values))), "NULL pointer");
-    const size_t esz = dtype == XRS_F64 || dtype == XRS_I64 ? 8 : (dtype == XRS_I16 || dtype == XRS_U16 ? 2 : 4);
-    XRS_REQUIRE(in_pitch >= W * (int64_t)esz && out_pitch >= W * (int64_t)(member ? esz : 4), "pitch below the row");
+    XRS_TRY(check_cells_arg(in, dtype, kRasterCells, in_pitch, W));
+    const size_t esz = cell_size(dtype);
+    XRS_TRY(check_out_pitch(out_pitch, member ? esz : 4, W));
     const size_t smem = (size_t)nb * (sizeof(double) + sizeof(float));
     const int in_smem = smem <= 96 * 1024 ? 1 : 0;   // else the lookup reads the table through L1 / L2
     const int64_t osz = member ? (int64_t)esz : 4;
@@ -732,7 +721,7 @@ int xrs_classify_cells(const void *in, int dtype, int64_t in_pitch, int64_t H, i
     const int64_t span = 2 * kThreads * (16 / (int64_t)esz);
     const int64_t tasks = H * ((W + span - 1) / span);
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(tasks, (int64_t)sm_count() * 8));
-    return with_cell_type(dtype, [&](auto t) -> int {
+    return with_cell_type(kRasterCells, dtype, [&](auto t) -> int {
         using T = decltype(t);
         auto kern = member ? classify_cells_kernel<T, true> : classify_cells_kernel<T, false>;
         const size_t sm = in_smem ? smem : 0;
@@ -752,10 +741,13 @@ int xrs_classify_moments(const void *in, int dtype, int64_t in_pitch, int64_t H,
                          double *out5, void *scratch, int64_t scratch_bytes, xrs_stream_t s) {
     XRS_REQUIRE(H >= 0 && W >= 0, "bad shape");
     XRS_REQUIRE(out5 && scratch && (in || H * W == 0), "NULL pointer");
-    XRS_REQUIRE(scratch_bytes >= (int64_t)sm_count() * 8 * (int64_t)sizeof(Moments), "scratch too small");
+    if (H * W) XRS_TRY(check_cells_arg(in, dtype, kRasterCells, in_pitch, W));
+    int64_t need = 0;
+    xrs_classify_moments_scratch_bytes(&need);
+    XRS_TRY(check_scratch(scratch, scratch_bytes, need, "xrs_classify_moments_scratch_bytes"));
     const int grid = grid_for(H, W, 8);
     Moments *part = static_cast<Moments *>(scratch);
-    int rc = with_cell_type(dtype, [&](auto t) -> int {
+    const int rc = with_cell_type(kRasterCells, dtype, [&](auto t) -> int {
         using T = decltype(t);
         moments_kernel<T><<<grid, kThreads, 0, (cudaStream_t)s>>>((const char *)in, in_pitch, H, W, above, part);
         XRS_CUDA(cudaGetLastError());
@@ -784,14 +776,15 @@ int xrs_classify_select(int source, const void *in, int dtype, int64_t in_pitch,
                 "NULL pointer");
     int64_t need = 0;
     xrs_classify_select_scratch_bytes(&need);
-    XRS_REQUIRE(scratch_bytes >= need, "scratch too small");
+    if (source == 0 && H * W) XRS_TRY(check_cells_arg(in, dtype, kRasterCells, in_pitch, W));
+    XRS_TRY(check_scratch(scratch, scratch_bytes, need, "xrs_classify_select_scratch_bytes"));
     if (nr) {
         int64_t n = 0;
         for (int d = 0; d < 256; ++d) n += (int64_t)hist0[d];
         for (int i = 0; i < nr; ++i) XRS_REQUIRE(ranks[i] >= 0 && ranks[i] < n, "rank outside the keys");
     }
     cudaStream_t st = (cudaStream_t)s;
-    return with_cell_type(dtype, [&](auto t) -> int {
+    return with_cell_type(kRasterCells, dtype, [&](auto t) -> int {
         using T = decltype(t);
         if (source == 0)
             return radix_select(CellKeys<T>{(const char *)in, in_pitch}, H, W, bits, ranks, nr, keys, rem, n_keys,
@@ -820,10 +813,11 @@ int xrs_classify_sort(const void *in, int dtype, int64_t in_pitch, int64_t H, in
     XRS_REQUIRE(keys && scratch && n_keys && (in || H * W == 0), "NULL pointer");
     int64_t need = 0;
     xrs_classify_sort_scratch_bytes(H * W, dtype, &need);
-    XRS_REQUIRE(scratch_bytes >= need, "scratch too small");
+    if (H * W) XRS_TRY(check_cells_arg(in, dtype, kRasterCells, in_pitch, W));
+    XRS_TRY(check_scratch(scratch, scratch_bytes, need, "xrs_classify_sort_scratch_bytes"));
     cudaStream_t st = (cudaStream_t)s;
     const int bits = key_bits(dtype);
-    return with_cell_type(dtype, [&](auto t) -> int {
+    return with_cell_type(kRasterCells, dtype, [&](auto t) -> int {
         using T = decltype(t);
         return with_key_type(dtype, [&](auto kt) -> int {
             using K = decltype(kt);
@@ -865,7 +859,7 @@ int xrs_classify_pick(const void *sorted, int dtype, int64_t n, int mode, uint64
     unsigned long long *dcount = static_cast<unsigned long long *>(scratch);
     XRS_CUDA(cudaMemsetAsync(dcount, 0, sizeof(unsigned long long), st));
     if (n) {
-        int rc = with_cell_type(dtype, [&](auto t) -> int {
+        int rc = with_cell_type(kRasterCells, dtype, [&](auto t) -> int {
             using T = decltype(t);
             return with_key_type(dtype, [&](auto kt) -> int {
                 using K = decltype(kt);

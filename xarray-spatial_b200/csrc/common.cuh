@@ -57,6 +57,13 @@ LaunchInfo &last_launch_info();
         }                                          \
     } while (0)
 
+// returns the status of a call that failed
+#define XRS_TRY(call)                  \
+    do {                               \
+        const int _rc = (call);        \
+        if (_rc != XRS_OK) return _rc; \
+    } while (0)
+
 // XRS_EINVAL with a message unless kh and kw are odd and 1 .. 2047: the windows of convolve and the focal
 // statistics (conv.cu)
 int check_window(int kh, int kw);
@@ -105,6 +112,94 @@ int launch(void (*kernel)(P...), int64_t grid, int threads, size_t smem, cudaStr
 // ...); callers then use kernels that load without TMA.
 bool make_tensor_map_2d(CUtensorMap *map, const void *base, int64_t pitch_bytes, int64_t H, int64_t W,
                         xrs_dtype dtype, int box_w, int box_h);
+
+// ----------------------------------------------------------------------------- raster arguments
+// Bytes per cell of an xrs_dtype code; 0 for an unknown code.
+inline int cell_size(int dtype) {
+    switch (dtype) {
+        case XRS_I8: case XRS_U8: case XRS_BOOL: return 1;
+        case XRS_I16: case XRS_U16: return 2;
+        case XRS_F32: case XRS_I32: case XRS_U32: return 4;
+        case XRS_F64: case XRS_I64: case XRS_U64: return 8;
+        default: return 0;
+    }
+}
+
+// The cell sets of xrs_b200.h: the raster set (F32, F64, I32, I64, I16, U16) and the zonal set (every code).
+struct RasterCells { static constexpr bool kAll = false; };
+struct ZonalCells { static constexpr bool kAll = true; };
+constexpr RasterCells kRasterCells{};
+constexpr ZonalCells kZonalCells{};
+
+template <class Set> bool in_cell_set(Set, int dtype) {
+    return Set::kAll ? cell_size(dtype) > 0 : (dtype >= XRS_F32 && dtype <= XRS_U16);
+}
+
+// Returns f(a value of dtype's C++ type) for a dtype in `set` (XRS_BOOL: bool), else XRS_EINVAL.
+template <class Set, class F> int with_cell_type(Set, int dtype, F &&f) {
+    switch (dtype) {
+        case XRS_F32: return f(float{});
+        case XRS_F64: return f(double{});
+        case XRS_I32: return f(int32_t{});
+        case XRS_I64: return f((long long)0);
+        case XRS_I16: return f(int16_t{});
+        case XRS_U16: return f(uint16_t{});
+    }
+    if constexpr (Set::kAll) {
+        switch (dtype) {
+            case XRS_I8: return f(int8_t{});
+            case XRS_U8: return f(uint8_t{});
+            case XRS_U32: return f(uint32_t{});
+            case XRS_U64: return f((unsigned long long)0);
+            case XRS_BOOL: return f(bool{});
+        }
+    }
+    set_error("unknown cell type %d", dtype);
+    return XRS_EINVAL;
+}
+
+// XRS_EINVAL unless `in` is set, dtype is in `set` and rows of W cells fit in_pitch bytes, a multiple of the cell
+// size (typed loads stay aligned).
+template <class Set> int check_cells_arg(const void *in, int dtype, Set set, int64_t in_pitch, int64_t W) {
+    XRS_REQUIRE(in != nullptr, "NULL input");
+    XRS_REQUIRE(in_cell_set(set, dtype), "unknown cell type");
+    const int64_t esz = cell_size(dtype);
+    XRS_REQUIRE(in_pitch % esz == 0 && in_pitch >= W * esz, "bad input pitch");
+    return XRS_OK;
+}
+
+// XRS_EINVAL unless rows of W cells of esz bytes fit out_pitch bytes, a multiple of esz.
+inline int check_out_pitch(int64_t out_pitch, int64_t esz, int64_t W) {
+    XRS_REQUIRE(out_pitch % esz == 0 && out_pitch >= W * esz, "bad output pitch");
+    return XRS_OK;
+}
+
+// XRS_EINVAL unless `scratch` is set and holds `need` bytes; `query` names the entry point that sizes it.
+inline int check_scratch(const void *scratch, int64_t bytes, int64_t need, const char *query) {
+    XRS_REQUIRE(scratch != nullptr, "NULL scratch buffer");
+    if (bytes < need) {
+        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (%s)", (long long)bytes,
+                  (long long)need, query);
+        return XRS_EINVAL;
+    }
+    return XRS_OK;
+}
+
+// Scratch regions start on 256-byte boundaries.
+constexpr int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
+
+// Grid of a 256-thread grid-stride loop over n items: at most 8 CTAs per SM, at least one.
+inline int64_t stride_grid(int64_t n) {
+    const int64_t g = (n + 255) / 256, cap = (int64_t)sm_count() * 8;
+    return g < 1 ? 1 : (g < cap ? g : cap);
+}
+
+// Cell (r, c) of a raster of T cells whose rows are `pitch` bytes apart.
+template <typename T> struct Cells {
+    const char *base;
+    int64_t pitch;
+    __device__ T operator()(int64_t r, int64_t c) const { return reinterpret_cast<const T *>(base + r * pitch)[c]; }
+};
 
 template <typename T> constexpr xrs_dtype dtype_of() {
     if constexpr (std::is_same_v<T, float>) return XRS_F32;

@@ -38,8 +38,6 @@ constexpr int kCompactThreads = 256, kCompactWords = 16;   // bitmap words per t
 constexpr int64_t kCompactTile = (int64_t)kCompactThreads * kCompactWords;
 static_assert(kChunk % (32 * kResolveUnroll) == 0, "the resolve reads whole groups of words");
 
-int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
-
 // The jump polynomials x^(kChunk 2^L) mod phi, L = 0 .. 15, computed once per process.
 constexpr int kMaxLevels = 16;
 std::once_flag g_poly_once;
@@ -314,10 +312,6 @@ __global__ void __launch_bounds__(kCompactThreads) nb_compact_kernel(const uint3
     }
 }
 
-int64_t stride_grid(int64_t n) {
-    return std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8));
-}
-
 int sample_args(int64_t n, int64_t s) {
     XRS_REQUIRE(n >= 1, "the sample needs at least one cell");
     if (n > ((int64_t)1 << 32)) {
@@ -400,13 +394,8 @@ extern "C" int xrs_nb_sample(int64_t n, int64_t s, uint32_t seed, int64_t *out, 
     int rc = sample_args(n, s);
     if (rc) return rc;
     XRS_REQUIRE(out != nullptr, "NULL output");
-    XRS_REQUIRE(scratch != nullptr, "NULL scratch buffer");
     const SampleLayout L(n, s);
-    if (scratch_bytes < L.total) {
-        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (xrs_nb_sample_scratch_bytes)",
-                  (long long)scratch_bytes, (long long)L.total);
-        return XRS_EINVAL;
-    }
+    XRS_TRY(check_scratch(scratch, scratch_bytes, L.total, "xrs_nb_sample_scratch_bytes"));
     if (L.levels > kMaxLevels) {
         set_error("xrs_nb_sample: %lld chunks need more than %d jump levels", (long long)L.chunks, kMaxLevels);
         return XRS_EINVAL;
@@ -515,11 +504,7 @@ extern "C" int xrs_nb_jenks(const float *x, int64_t n, int k, float *lcl, void *
     XRS_REQUIRE(x != nullptr && lcl != nullptr && scratch != nullptr, "NULL pointer");
     int64_t need = 0;
     xrs_nb_jenks_scratch_bytes(n, k, &need);
-    if (scratch_bytes < need) {
-        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (xrs_nb_jenks_scratch_bytes)",
-                  (long long)scratch_bytes, (long long)need);
-        return XRS_EINVAL;
-    }
+    XRS_TRY(check_scratch(scratch, scratch_bytes, need, "xrs_nb_jenks_scratch_bytes"));
     cudaStream_t st = (cudaStream_t)stream;
     float *var = (float *)scratch;
     nb_jenks_init_kernel<<<(unsigned)stride_grid((int64_t)(k + 1) * (n + 1)), 256, 0, st>>>(n, k, lcl, var);

@@ -38,8 +38,6 @@ struct TableCtl {
 };
 static_assert(sizeof(TableCtl) <= kCtl, "control block");
 
-int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
-
 struct TableLayout {
     int64_t mt, words, step, J, R, list0, list1, total;
     TableLayout(int S, int64_t n) {
@@ -156,8 +154,6 @@ __global__ void nz_commit_kernel(const int32_t *list_in, const int *count_in, in
         }
     }
 }
-
-int64_t stride_grid(int64_t n) { return std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8)); }
 
 int table_args(int n_seeds, int64_t n) {
     XRS_REQUIRE(n_seeds >= 1 && n_seeds <= kMaxSeeds, "n_seeds must be 1 .. 32");
@@ -419,13 +415,8 @@ extern "C" int xrs_perm_tables(const uint32_t *seeds, int n_seeds, int64_t n, in
     if (rc) return rc;
     XRS_REQUIRE(seeds != nullptr, "NULL seed list");
     XRS_REQUIRE(tables != nullptr, "NULL tables");
-    XRS_REQUIRE(scratch != nullptr, "NULL scratch buffer");
     const TableLayout L(n_seeds, n);
-    if (scratch_bytes < L.total) {
-        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (xrs_perm_tables_scratch_bytes)",
-                  (long long)scratch_bytes, (long long)L.total);
-        return XRS_EINVAL;
-    }
+    XRS_TRY(check_scratch(scratch, scratch_bytes, L.total, "xrs_perm_tables_scratch_bytes"));
     cudaStream_t s = (cudaStream_t)stream;
     char *sc = (char *)scratch;
     TableCtl *ctl = (TableCtl *)sc;
@@ -509,20 +500,13 @@ extern "C" int xrs_noise(const void *in, int dtype, int64_t in_pitch, int64_t H,
     int rc = noise_shape(H, W);
     if (rc) return rc;
     XRS_REQUIRE(dtype == XRS_F32 || dtype == XRS_F64, "the noise functions take float32 or float64 cells");
-    const int64_t esz = dtype == XRS_F32 ? 4 : 8;
-    XRS_REQUIRE(!terrain || in != nullptr, "NULL input");
-    XRS_REQUIRE(!terrain || (in_pitch % esz == 0 && in_pitch >= W * esz), "bad input pitch");
+    if (terrain) XRS_TRY(check_cells_arg(in, dtype, kRasterCells, in_pitch, W));
     XRS_REQUIRE(tables != nullptr && xs != nullptr && ys != nullptr, "NULL tables or coordinates");
     XRS_REQUIRE(out != nullptr, "NULL output");
-    XRS_REQUIRE(out_pitch % esz == 0 && out_pitch >= W * esz, "bad output pitch");
+    XRS_TRY(check_out_pitch(out_pitch, cell_size(dtype), W));
     XRS_REQUIRE(index_stats != nullptr, "NULL index_stats");
-    XRS_REQUIRE(scratch != nullptr, "NULL scratch buffer");
     const NoiseLayout L(H, W, terrain ? kTerrainOctaves : 1);
-    if (scratch_bytes < L.total) {
-        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (xrs_noise_scratch_bytes)",
-                  (long long)scratch_bytes, (long long)L.total);
-        return XRS_EINVAL;
-    }
+    XRS_TRY(check_scratch(scratch, scratch_bytes, L.total, "xrs_noise_scratch_bytes"));
     cudaStream_t s = (cudaStream_t)stream;
     char *sc = (char *)scratch;
     if (dtype == XRS_F32) {

@@ -36,7 +36,7 @@ struct Barriers {
 
 template <typename T> __device__ __forceinline__ bool crossable(const void *in, int64_t pitch, int64_t r, int64_t c,
                                                                 const Barriers &bar) {
-    const double v = (double)reinterpret_cast<const T *>((const char *)in + r * pitch)[c];   // as NumPy compares
+    const double v = (double)Cells<T>{(const char *)in, pitch}(r, c);   // as NumPy compares
     if (v != v) return false;
     for (int i = 0; i < bar.n; ++i)
         if (v == bar.v[i]) return false;
@@ -233,8 +233,6 @@ __global__ void pf_snap_idx_kernel(const void *in, int64_t pitch, int64_t H, int
     }
 }
 
-int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
-
 struct Layout {
     int64_t tiles_x, tiles_y, ntiles, dist, mask, stamp, list0, list1, total;
     Layout(int64_t H, int64_t W) {
@@ -261,32 +259,10 @@ int check_shape(int64_t H, int64_t W) {
 }
 
 int check_cells(const void *in, int in_dtype, int64_t in_pitch, int64_t W, const double *barriers, int n_barriers) {
-    XRS_REQUIRE(in != nullptr, "NULL input");
-    int esz = 0;
-    switch (in_dtype) {
-        case XRS_F32: case XRS_I32: esz = 4; break;
-        case XRS_F64: case XRS_I64: esz = 8; break;
-        case XRS_I16: case XRS_U16: esz = 2; break;
-        default: XRS_REQUIRE(false, "unknown cell type");
-    }
-    XRS_REQUIRE(in_pitch % esz == 0 && in_pitch >= W * esz, "bad input pitch");
+    XRS_TRY(check_cells_arg(in, in_dtype, kRasterCells, in_pitch, W));
     XRS_REQUIRE(n_barriers >= 0 && (n_barriers == 0 || barriers != nullptr), "bad barrier list");
     return XRS_OK;
 }
-
-// Calls f.template operator()<T>() with the C++ type of in_dtype.
-template <class F> int by_dtype(int in_dtype, F &&f) {
-    switch (in_dtype) {
-        case XRS_F32: return f((float)0);
-        case XRS_F64: return f((double)0);
-        case XRS_I32: return f((int)0);
-        case XRS_I64: return f((long long)0);
-        case XRS_I16: return f((short)0);
-        default: return f((unsigned short)0);
-    }
-}
-
-int64_t stride_grid(int64_t n) { return std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8); }
 
 // The distance field from the goal: the mask pass, then batches of kBatch rounds with one read of the activity
 // counts per batch.  At most H W + 1 rounds change a cell (a shortest path crosses fewer tile borders than it has
@@ -372,21 +348,16 @@ extern "C" int xrs_a_star_search(const void *in, int in_dtype, int64_t in_pitch,
     XRS_REQUIRE(start_row >= 0 && start_row < H && start_col >= 0 && start_col < W, "start outside the raster");
     XRS_REQUIRE(goal_row >= 0 && goal_row < H && goal_col >= 0 && goal_col < W, "goal outside the raster");
     XRS_REQUIRE(out != nullptr, "NULL output");
-    XRS_REQUIRE(out_pitch % 8 == 0 && out_pitch >= W * 8, "bad output pitch");
-    XRS_REQUIRE(scratch != nullptr, "NULL scratch buffer");
+    XRS_TRY(check_out_pitch(out_pitch, 8, W));
     const Layout L(H, W);
-    if (scratch_bytes < L.total) {
-        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (xrs_a_star_scratch_bytes)",
-                  (long long)scratch_bytes, (long long)L.total);
-        return XRS_EINVAL;
-    }
+    XRS_TRY(check_scratch(scratch, scratch_bytes, L.total, "xrs_a_star_scratch_bytes"));
     cudaStream_t st = (cudaStream_t)s;
     char *sc = (char *)scratch;
     const Field f{(Dist *)(sc + L.dist), (const uint8_t *)(sc + L.mask), (int)H, (int)W, connectivity,
                   (int)L.tiles_x, (int)L.tiles_y, (int)goal_row, (int)goal_col};
     const Barriers bar{barriers, n_barriers};
     int64_t nrounds = 0;
-    rc = by_dtype(in_dtype, [&](auto z) {
+    rc = with_cell_type(kRasterCells, in_dtype, [&](auto z) {
         return build_field<decltype(z)>(in, in_pitch, bar, f, L, sc, &nrounds, st);
     });
     if (rc) return rc;
@@ -423,7 +394,7 @@ extern "C" int xrs_a_star_snap(const void *in, int in_dtype, int64_t in_pitch, i
     XRS_CUDA(cudaMemsetAsync(&ctl->snap_d2, 0xff, 16, st));
     const Barriers bar{barriers, n_barriers};
     const unsigned grid = (unsigned)stride_grid(H * W);
-    rc = by_dtype(in_dtype, [&](auto z) -> int {
+    rc = with_cell_type(kRasterCells, in_dtype, [&](auto z) -> int {
         using T = decltype(z);
         pf_snap_d2_kernel<T><<<grid, 256, 0, st>>>(in, in_pitch, H, W, bar, row, col, &ctl->snap_d2);
         XRS_CUDA(cudaGetLastError());

@@ -32,10 +32,6 @@ template <typename T> __device__ __forceinline__ bool is_target(T raw, const Tar
     return a < rule.n && rule.values[a] == v;
 }
 
-template <typename T> __device__ __forceinline__ T load_cell(const void *in, int64_t pitch, int64_t r, int64_t c) {
-    return reinterpret_cast<const T *>(reinterpret_cast<const char *>(in) + r * pitch)[c];
-}
-
 // The row pass key of target column t for cell column c: smaller is nearer.
 template <int M> __device__ __forceinline__ double row_key(const double *X, const double *lam, int t, int c) {
     if (M == kGreatCircle) return -cos(lam[t] - lam[c]);   // the haversine grows with 1 - cos(dlon)
@@ -61,7 +57,7 @@ __global__ void __launch_bounds__(kRowThreads) prox_row_kernel(const void *in, i
     __syncthreads();
     for (int k = ntiles - 1; k >= 0; --k) {
         const int c = k * kRowThreads + tid;
-        const bool tg = c < W && is_target(load_cell<T>(in, in_pitch, r, c), rule);
+        const bool tg = c < W && is_target(Cells<T>{(const char *)in, in_pitch}(r, c), rule);
         int v = tg ? c : kNoTarget;
         if (M == kGreatCircle) {
             const int mx = __reduce_max_sync(0xffffffffu, tg ? c : -1);
@@ -203,7 +199,7 @@ template <typename T, int M> __global__ void prox_query_kernel(Column<M> proto, 
             const float sq = f * f;   // the reference keeps the squared float32 distance
             if (self || md2 >= (double)sq) {
                 if (a.mode == XRS_PROX_DISTANCE) res = self ? 0.0f : (float)sqrt((double)sq);
-                else if (a.mode == XRS_PROX_ALLOCATION) res = (float)load_cell<T>(a.in, a.in_pitch, r, t);
+                else if (a.mode == XRS_PROX_ALLOCATION) res = (float)Cells<T>{(const char *)a.in, a.in_pitch}(r, t);
                 else res = self ? 0.0f : direction_deg(xc, xt, yc, yt);
             }
         }
@@ -216,8 +212,6 @@ template <typename T, int M> __global__ void prox_query_kernel(Column<M> proto, 
 struct Layout {
     int64_t band_rows, nb, ridx, stk, blo, bhi, bprev, boff, cosl, sinl, lam, total;
 };
-
-int64_t align256(int64_t v) { return (v + 255) & ~int64_t(255); }
 
 Layout layout(int64_t H, int64_t W, int64_t band_rows) {
     Layout L;
@@ -336,31 +330,13 @@ extern "C" int xrs_proximity(const void *in, int in_dtype, int64_t in_pitch, int
     XRS_REQUIRE(n_targets >= 0 && (n_targets == 0 || targets != nullptr), "bad target list");
     if (H == 0 || W == 0) return XRS_OK;
     XRS_REQUIRE(in && out && x && y, "NULL pointer");
-    int esz = 0;
-    switch (in_dtype) {
-        case XRS_F32: case XRS_I32: esz = 4; break;
-        case XRS_F64: case XRS_I64: esz = 8; break;
-        case XRS_I16: case XRS_U16: esz = 2; break;
-        default: XRS_REQUIRE(false, "unknown cell type");
-    }
-    XRS_REQUIRE(in_pitch % esz == 0 && in_pitch >= W * esz, "bad input pitch");
-    XRS_REQUIRE(out_pitch % 4 == 0 && out_pitch >= W * 4, "bad output pitch");
+    XRS_TRY(check_cells_arg(in, in_dtype, kRasterCells, in_pitch, W));
+    XRS_TRY(check_out_pitch(out_pitch, 4, W));
     const Layout L = layout(H, W, band_rows);
-    XRS_REQUIRE(scratch != nullptr, "NULL scratch buffer");
-    if (scratch_bytes < L.total) {
-        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (xrs_proximity_scratch_bytes)",
-                  (long long)scratch_bytes, (long long)L.total);
-        return XRS_EINVAL;
-    }
+    XRS_TRY(check_scratch(scratch, scratch_bytes, L.total, "xrs_proximity_scratch_bytes"));
     const TargetRule rule{targets, n_targets};
-    cudaStream_t st = (cudaStream_t)s;
-    char *sc = (char *)scratch;
-    switch (in_dtype) {
-        case XRS_F32: return run_metric<float>(metric, in, in_pitch, H, W, x, y, rule, max_distance, mode, out, out_pitch, sc, L, st);
-        case XRS_F64: return run_metric<double>(metric, in, in_pitch, H, W, x, y, rule, max_distance, mode, out, out_pitch, sc, L, st);
-        case XRS_I32: return run_metric<int>(metric, in, in_pitch, H, W, x, y, rule, max_distance, mode, out, out_pitch, sc, L, st);
-        case XRS_I64: return run_metric<long long>(metric, in, in_pitch, H, W, x, y, rule, max_distance, mode, out, out_pitch, sc, L, st);
-        case XRS_I16: return run_metric<short>(metric, in, in_pitch, H, W, x, y, rule, max_distance, mode, out, out_pitch, sc, L, st);
-        default: return run_metric<unsigned short>(metric, in, in_pitch, H, W, x, y, rule, max_distance, mode, out, out_pitch, sc, L, st);
-    }
+    return with_cell_type(kRasterCells, in_dtype, [&](auto z) {
+        return run_metric<decltype(z)>(metric, in, in_pitch, H, W, x, y, rule, max_distance, mode, out, out_pitch,
+                                       (char *)scratch, L, (cudaStream_t)s);
+    });
 }

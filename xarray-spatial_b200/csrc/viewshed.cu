@@ -14,20 +14,12 @@ using namespace vs;
 
 constexpr int kTile = 16;   // the visibility pass gives each 16 x 16 block a tile of targets with similar rays
 
-template <typename T> struct Cells {
-    const char *base;
-    int64_t pitch;
-    __device__ double operator()(int64_t r, int64_t c) const {
-        return (double)reinterpret_cast<const T *>(base + r * pitch)[c];
-    }
-};
-
 template <typename T> __global__ void vs_node_kernel(View v, Cells<T> z, Node *nodes) {
     const int64_t n = v.H * v.W;
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) {
         const int64_t r = k / v.W, c = k - r * v.W;
         if (r == v.vr && c == v.vc) continue;   // the observer has no node
-        nodes[k] = make_node(v, z, r, c);
+        nodes[k] = make_node(v, [&](int64_t rr, int64_t cc) { return (double)z(rr, cc); }, r, c);
     }
 }
 
@@ -84,30 +76,11 @@ extern "C" int xrs_viewshed(const void *in, int in_dtype, int64_t in_pitch, int6
     XRS_REQUIRE(H > 0 && W > 0, "viewshed needs a raster of at least one cell");
     XRS_REQUIRE(vp_row >= 0 && vp_row < H && vp_col >= 0 && vp_col < W, "observer outside the raster");
     XRS_REQUIRE(in && out, "NULL pointer");
-    int esz = 0;
-    switch (in_dtype) {
-        case XRS_F32: case XRS_I32: esz = 4; break;
-        case XRS_F64: case XRS_I64: esz = 8; break;
-        case XRS_I16: case XRS_U16: esz = 2; break;
-        default: XRS_REQUIRE(false, "unknown cell type");
-    }
-    XRS_REQUIRE(in_pitch % esz == 0 && in_pitch >= W * esz, "bad input pitch");
-    XRS_REQUIRE(out_pitch % 8 == 0 && out_pitch >= W * 8, "bad output pitch");
-    XRS_REQUIRE(scratch != nullptr, "NULL scratch buffer");
-    if (scratch_bytes < scratch_need(H, W)) {
-        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (xrs_viewshed_scratch_bytes)",
-                  (long long)scratch_bytes, (long long)scratch_need(H, W));
-        return XRS_EINVAL;
-    }
+    XRS_TRY(check_cells_arg(in, in_dtype, kRasterCells, in_pitch, W));
+    XRS_TRY(check_out_pitch(out_pitch, 8, W));
+    XRS_TRY(check_scratch(scratch, scratch_bytes, scratch_need(H, W), "xrs_viewshed_scratch_bytes"));
     const View v{H, W, vp_row, vp_col, vp_elev, target_elev, ew_res, ns_res};
-    cudaStream_t st = (cudaStream_t)s;
-    Node *nodes = (Node *)scratch;
-    switch (in_dtype) {
-        case XRS_F32: return run<float>(v, in, in_pitch, out, out_pitch, nodes, st);
-        case XRS_F64: return run<double>(v, in, in_pitch, out, out_pitch, nodes, st);
-        case XRS_I32: return run<int>(v, in, in_pitch, out, out_pitch, nodes, st);
-        case XRS_I64: return run<long long>(v, in, in_pitch, out, out_pitch, nodes, st);
-        case XRS_I16: return run<short>(v, in, in_pitch, out, out_pitch, nodes, st);
-        default: return run<unsigned short>(v, in, in_pitch, out, out_pitch, nodes, st);
-    }
+    return with_cell_type(kRasterCells, in_dtype, [&](auto z) {
+        return run<decltype(z)>(v, in, in_pitch, out, out_pitch, (Node *)scratch, (cudaStream_t)s);
+    });
 }

@@ -21,12 +21,6 @@ constexpr int kScanThreads = 256;
 constexpr int kScanPer = 16;             // cells per thread of the numbering passes
 constexpr int64_t kScanChunk = (int64_t)kScanThreads * kScanPer;
 
-template <typename T> struct Cells {
-    const char *base;
-    int64_t pitch;
-    __device__ T operator()(int64_t r, int64_t c) const { return reinterpret_cast<const T *>(base + r * pitch)[c]; }
-};
-
 __device__ __forceinline__ int ld_cg(const int *p) { return __ldcg(p); }
 __device__ __forceinline__ long long ld_cg(const long long *p) { return __ldcg(p); }
 
@@ -224,8 +218,6 @@ __global__ void zr_label_kernel(const uint16_t *code, const Idx *parent, const I
     }
 }
 
-constexpr int64_t align256(int64_t b) { return (b + 255) / 256 * 256; }
-
 bool wide_index(int64_t N) { return N > (int64_t)INT32_MAX; }
 
 int64_t regions_need(int64_t H, int64_t W) {
@@ -274,16 +266,6 @@ int regions_typed(const void *in, int64_t in_pitch, int64_t H, int64_t W, int n,
     if (wide_index(H * W))
         return regions_run<T, OutT, long long>(in, in_pitch, H, W, n, out, out_pitch, scratch, s);
     return regions_run<T, OutT, int>(in, in_pitch, H, W, n, out, out_pitch, scratch, s);
-}
-
-int cell_size(int dtype) {
-    switch (dtype) {
-        case XRS_I8: case XRS_U8: case XRS_BOOL: return 1;
-        case XRS_I16: case XRS_U16: return 2;
-        case XRS_F32: case XRS_I32: case XRS_U32: return 4;
-        case XRS_F64: case XRS_I64: case XRS_U64: return 8;
-        default: return 0;
-    }
 }
 
 int check_shape(int64_t H, int64_t W) {
@@ -388,34 +370,21 @@ extern "C" int xrs_zonal_regions(const void *in, int dtype, int64_t in_pitch, in
     int rc = check_shape(H, W);
     if (rc) return rc;
     XRS_REQUIRE(neighborhood == 4 || neighborhood == 8, "neighborhood must be 4 or 8");
-    const int esz = cell_size(dtype);
-    XRS_REQUIRE(esz > 0, "unknown cell type");
+    XRS_REQUIRE(in_cell_set(kZonalCells, dtype), "unknown cell type");
     if (H == 0 || W == 0) return XRS_OK;
     XRS_REQUIRE(in && out, "NULL pointer");
-    XRS_REQUIRE(in_pitch % esz == 0 && in_pitch >= W * esz, "bad input pitch");
-    XRS_REQUIRE(out_pitch % esz == 0 && out_pitch >= W * esz, "bad output pitch");
-    XRS_REQUIRE(scratch != nullptr, "NULL scratch buffer");
-    if (scratch_bytes < regions_need(H, W)) {
-        set_error("scratch buffer of %lld bytes is too small: this call needs %lld (xrs_zonal_regions_scratch_bytes)",
-                  (long long)scratch_bytes, (long long)regions_need(H, W));
-        return XRS_EINVAL;
-    }
-    cudaStream_t st = (cudaStream_t)s;
-    char *sc = (char *)scratch;
-    const int n = neighborhood;
-    switch (dtype) {
-        case XRS_F32: return regions_typed<float>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_F64: return regions_typed<double>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_I8: return regions_typed<int8_t>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_I16: return regions_typed<int16_t>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_I32: return regions_typed<int32_t>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_I64: return regions_typed<long long>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_U8: return regions_typed<uint8_t>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_U16: return regions_typed<uint16_t>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_U32: return regions_typed<uint32_t>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        case XRS_U64: return regions_typed<unsigned long long>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-        default: return regions_typed<uint8_t, bool>(in, in_pitch, H, W, n, out, out_pitch, sc, st);
-    }
+    XRS_TRY(check_cells_arg(in, dtype, kZonalCells, in_pitch, W));
+    XRS_TRY(check_out_pitch(out_pitch, cell_size(dtype), W));
+    XRS_TRY(check_scratch(scratch, scratch_bytes, regions_need(H, W), "xrs_zonal_regions_scratch_bytes"));
+    return with_cell_type(kZonalCells, dtype, [&](auto z) {
+        using T = decltype(z);
+        const int n = neighborhood;
+        char *sc = (char *)scratch;
+        if constexpr (std::is_same_v<T, bool>)   // bool cells are read as uint8 and labelled as bool
+            return regions_typed<uint8_t, bool>(in, in_pitch, H, W, n, out, out_pitch, sc, (cudaStream_t)s);
+        else
+            return regions_typed<T>(in, in_pitch, H, W, n, out, out_pitch, sc, (cudaStream_t)s);
+    });
 }
 
 extern "C" int xrs_zonal_bounds(const void *in, int dtype, int64_t in_pitch, int64_t H, int64_t W, int mode,
@@ -424,26 +393,15 @@ extern "C" int xrs_zonal_bounds(const void *in, int dtype, int64_t in_pitch, int
     int rc = check_shape(H, W);
     if (rc) return rc;
     XRS_REQUIRE(mode == 0 || mode == 1, "mode must be 0 (trim) or 1 (crop)");
-    const int esz = cell_size(dtype);
-    XRS_REQUIRE(esz > 0, "unknown cell type");
+    XRS_REQUIRE(in_cell_set(kZonalCells, dtype), "unknown cell type");
     XRS_REQUIRE(n_values >= 0, "negative value count");
     XRS_REQUIRE(out4 != nullptr, "NULL pointer");
     XRS_REQUIRE(H == 0 || W == 0 || in != nullptr, "NULL pointer");
     XRS_REQUIRE(n_values == 0 || values != nullptr, "NULL values");
-    XRS_REQUIRE(H == 0 || W == 0 || (in_pitch % esz == 0 && in_pitch >= W * esz), "bad input pitch");
+    if (H && W) XRS_TRY(check_cells_arg(in, dtype, kZonalCells, in_pitch, W));
     const Targets t{values, (const long long *)int_values, n_values, int_values != nullptr};
-    cudaStream_t st = (cudaStream_t)s;
-    long long *o = (long long *)out4;
-    switch (dtype) {
-        case XRS_F32: return bounds_typed<float>(in, in_pitch, H, W, mode, t, o, st);
-        case XRS_F64: return bounds_typed<double>(in, in_pitch, H, W, mode, t, o, st);
-        case XRS_I8: return bounds_typed<int8_t>(in, in_pitch, H, W, mode, t, o, st);
-        case XRS_I16: return bounds_typed<int16_t>(in, in_pitch, H, W, mode, t, o, st);
-        case XRS_I32: return bounds_typed<int32_t>(in, in_pitch, H, W, mode, t, o, st);
-        case XRS_I64: return bounds_typed<long long>(in, in_pitch, H, W, mode, t, o, st);
-        case XRS_U16: return bounds_typed<uint16_t>(in, in_pitch, H, W, mode, t, o, st);
-        case XRS_U32: return bounds_typed<uint32_t>(in, in_pitch, H, W, mode, t, o, st);
-        case XRS_U64: return bounds_typed<unsigned long long>(in, in_pitch, H, W, mode, t, o, st);
-        default: return bounds_typed<uint8_t>(in, in_pitch, H, W, mode, t, o, st);   // uint8, bool
-    }
+    return with_cell_type(kZonalCells, dtype, [&](auto z) {
+        using T = std::conditional_t<std::is_same_v<decltype(z), bool>, uint8_t, decltype(z)>;   // bool as uint8
+        return bounds_typed<T>(in, in_pitch, H, W, mode, t, (long long *)out4, (cudaStream_t)s);
+    });
 }

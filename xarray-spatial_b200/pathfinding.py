@@ -19,23 +19,17 @@ import numpy as np
 
 from . import _lib
 from ._xr import DataArray
-from .proximity import _cells
-from .utils import as_device_tensor, get_dataarray_resolution, is_dask_array, is_device_array, like_container
-from .utils import stream_ptr
+from .utils import as_device_tensor, call_on, coord, device_cells, device_scratch, get_dataarray_resolution
+from .utils import is_dask_array, is_device_array, pitch, ptr, to_container
 
 NONE = -1
-
-
-def _coord(raster, name):
-    c = raster[name]
-    return np.asarray(getattr(c, "data", c))
 
 
 def _get_pixel_id(point, raster, xdim, ydim):
     """The (row, column) of a (y, x) point: int(|p - coord[0]| / cellsize) along each axis."""
     cellsize_x, cellsize_y = get_dataarray_resolution(raster, xdim, ydim)
-    py = int(abs(point[0] - _coord(raster, ydim)[0]) / cellsize_y)
-    px = int(abs(point[1] - _coord(raster, xdim)[0]) / cellsize_x)
+    py = int(abs(point[0] - coord(raster, ydim)[0]) / cellsize_y)
+    px = int(abs(point[1] - coord(raster, xdim)[0]) / cellsize_x)
     return py, px
 
 
@@ -108,11 +102,10 @@ def a_star_search(surface, start, goal, barriers=[], x="x", y="y", connectivity=
 
     def cells(bars):   # the raster on the device and the C arguments that describe it and the barriers
         if "t" not in dev:
-            dev["t"], code = _cells(data)
+            dev["t"], code = device_cells(data, "a_star_search", "widen")
             t = dev["t"]
             dev["bars"] = torch.as_tensor(np.append(bars, 0.0), device=t.device)   # never a NULL pointer
-            dev["args"] = (ctypes.c_void_p(t.data_ptr()), code, t.stride(0) * t.element_size(), t.shape[0],
-                           t.shape[1], ctypes.c_void_p(dev["bars"].data_ptr()), bars.size)
+            dev["args"] = (ptr(t), code, pitch(t), t.shape[0], t.shape[1], ptr(dev["bars"]), bars.size)
         return dev["t"], dev["args"]
 
     def cell(py, px):
@@ -124,29 +117,20 @@ def a_star_search(surface, start, goal, barriers=[], x="x", y="y", connectivity=
         t, args = cells(bars)
         r, c = ctypes.c_int64(), ctypes.c_int64()
         scratch = torch.empty(256, dtype=torch.uint8, device=t.device)
-        with torch.cuda.device(t.device):
-            _lib.call("xrs_a_star_snap", *args, py, px, ctypes.byref(r), ctypes.byref(c),
-                      ctypes.c_void_p(scratch.data_ptr()), 256, stream_ptr(t))
+        call_on(t, "xrs_a_star_snap", *args, py, px, ctypes.byref(r), ctypes.byref(c), ptr(scratch), 256)
         return r.value, c.value
 
     bars, cells_of_path = _plan(surface, start, goal, barriers, x, y, connectivity, snap_start, snap_goal, cell,
                                 snap)
     t, args = cells(bars)
     H, W = t.shape
-    need = ctypes.c_int64()
-    _lib.call("xrs_a_star_scratch_bytes", H, W, ctypes.byref(need))
     if cells_of_path is None:
+        _lib.call("xrs_a_star_scratch_bytes", H, W, ctypes.byref(ctypes.c_int64()))   # the raster's size limit
         out = torch.full((H, W), float("nan"), dtype=torch.float64, device=t.device)
     else:
         (sr, sc), (gr, gc) = cells_of_path
-        try:
-            scratch = torch.empty(need.value, dtype=torch.uint8, device=t.device)
-        except torch.OutOfMemoryError as e:
-            raise MemoryError("a_star_search needs %d bytes of device scratch for a %d x %d raster"
-                              % (need.value, H, W)) from e
+        scratch, size = device_scratch("xrs_a_star_scratch_bytes", H, W, device=t.device, what="a_star_search")
         out = torch.empty((H, W), dtype=torch.float64, device=t.device)
-        with torch.cuda.device(t.device):
-            _lib.call("xrs_a_star_search", *args, connectivity, sr, sc, gr, gc, ctypes.c_void_p(out.data_ptr()),
-                      out.stride(0) * 8, ctypes.c_void_p(scratch.data_ptr()), need.value, None, stream_ptr(t))
-    result = out.cpu().numpy() if isinstance(data, np.ndarray) else like_container(out, data)
-    return DataArray(result, coords=surface.coords, dims=surface.dims, attrs=surface.attrs)
+        call_on(t, "xrs_a_star_search", *args, connectivity, sr, sc, gr, gc, ptr(out), pitch(out), ptr(scratch),
+                size, None)
+    return DataArray(to_container(out, data), coords=surface.coords, dims=surface.dims, attrs=surface.attrs)

@@ -19,15 +19,13 @@ import operator
 
 import numpy as np
 
-from . import _lib
 from ._xr import DataArray
-from .utils import as_device_tensor, host_device_index, is_dask_array, is_device_array, like_container
-from .utils import stream_ptr
+from .utils import call_on, device_2d, device_scratch, host_device_index, is_dask_array, ptr, raster_cells
+from .utils import to_container
 
 TABLE_N = 2 ** 20          # the reference's permutation(2**20)
 INDEX_LIMIT = 2 ** 21      # np.append(p, p) takes indices in [-2**21, 2**21)
 TERRAIN_OCTAVES = 16
-_CODES = {"float32": 0, "float64": 1}
 
 
 def check_seed(seed, count=1):
@@ -42,23 +40,9 @@ def check_seed(seed, count=1):
 
 
 def check_cells(data, fname):
-    """A numpy or device raster of float32 / float64 cells with at least one cell; returns its dtype name."""
-    if is_dask_array(data):
-        raise NotImplementedError("%s: Dask arrays are not supported by the GPU backend" % fname)
-    if isinstance(data, np.ndarray):
-        dtype, shape = str(data.dtype), data.shape
-    elif is_device_array(data):
-        t = as_device_tensor(data)
-        dtype, shape = str(t.dtype).replace("torch.", ""), tuple(t.shape)
-    else:
-        raise TypeError("Unsupported raster array type: {}".format(type(data)))
-    if len(shape) != 2:
-        raise ValueError("%s needs a 2-D raster, got %d-D" % (fname, len(shape)))
-    if dtype not in _CODES:
-        raise TypeError("%s takes float32 or float64 cells, not %s" % (fname, dtype))
-    if shape[0] == 0 or shape[1] == 0:
+    """A numpy or device raster of float32 / float64 cells with at least one cell."""
+    if 0 in raster_cells(data, fname, "float")[0].shape:
         raise ValueError("zero-size array to reduction operation minimum which has no identity")
-    return dtype
 
 
 def perm_tables(seeds, device, rounds=None):
@@ -66,16 +50,13 @@ def perm_tables(seeds, device, rounds=None):
     there on torch's current stream."""
     import torch
     n = TABLE_N
-    need = ctypes.c_int64()
-    _lib.call("xrs_perm_tables_scratch_bytes", len(seeds), n, ctypes.byref(need))
     tables = torch.empty((len(seeds), n), dtype=torch.int32, device=device)
-    scratch = torch.empty(need.value, dtype=torch.uint8, device=device)
+    scratch, size = device_scratch("xrs_perm_tables_scratch_bytes", len(seeds), n, device=device,
+                                   what="the permutation tables")
     host = (ctypes.c_uint32 * len(seeds))(*seeds)
     r = ctypes.c_int64()
-    with torch.cuda.device(device):
-        _lib.call("xrs_perm_tables", ctypes.cast(host, ctypes.c_void_p), len(seeds), n,
-                  ctypes.c_void_p(tables.data_ptr()), ctypes.c_void_p(scratch.data_ptr()), need.value,
-                  ctypes.byref(r), stream_ptr(tables))
+    call_on(tables, "xrs_perm_tables", ctypes.cast(host, ctypes.c_void_p), len(seeds), n, ptr(tables), ptr(scratch),
+            size, ctypes.byref(r))
     if rounds is not None:
         rounds.append(r.value)
     return tables
@@ -99,9 +80,7 @@ def run_noise(data, seeds, xs, ys, terrain, zfactor=0.0):
         device = torch.device("cuda", host_device_index())
         t = torch.from_numpy(np.ascontiguousarray(data)).to(device) if terrain else None
     else:
-        t = as_device_tensor(data)
-        if t.stride(1) != 1:
-            t = t.contiguous()
+        t = device_2d(data)
         device = t.device
     H, W = data.shape
     dtype = torch.float32 if str(data.dtype).endswith("float32") else torch.float64
@@ -110,24 +89,21 @@ def run_noise(data, seeds, xs, ys, terrain, zfactor=0.0):
         tables = perm_tables(seeds, device)
         dx = torch.from_numpy(np.ascontiguousarray(xs, dtype=np.float32)).to(device)
         dy = torch.from_numpy(np.ascontiguousarray(ys, dtype=np.float32)).to(device)
-        need = ctypes.c_int64()
-        _lib.call("xrs_noise_scratch_bytes", H, W, int(terrain), ctypes.byref(need))
+        scratch, size = device_scratch("xrs_noise_scratch_bytes", H, W, int(terrain), device=device,
+                                       what="the noise of a %d x %d raster" % (H, W))
         try:
-            scratch = torch.empty(need.value, dtype=torch.uint8, device=device)
             out = torch.empty((H, W), dtype=dtype, device=device)
         except torch.OutOfMemoryError as e:
-            raise MemoryError("the noise of a %d x %d raster needs %d bytes of device scratch"
-                              % (H, W, need.value)) from e
+            raise MemoryError("the noise of a %d x %d raster needs %d bytes of device memory"
+                              % (H, W, H * W * (4 if code == 0 else 8))) from e
         stats = torch.empty((len(seeds), 5), dtype=torch.int32, device=device)
         esz = out.element_size()
-        _lib.call("xrs_noise", ctypes.c_void_p(t.data_ptr() if t is not None else 0), code,
-                  t.stride(0) * esz if t is not None else 0, H, W, ctypes.c_void_p(tables.data_ptr()),
-                  ctypes.c_void_p(dx.data_ptr()), ctypes.c_void_p(dy.data_ptr()), int(terrain), float(zfactor),
-                  ctypes.c_void_p(out.data_ptr()), out.stride(0) * esz, ctypes.c_void_p(stats.data_ptr()),
-                  ctypes.c_void_p(scratch.data_ptr()), need.value, stream_ptr(out))
+        call_on(out, "xrs_noise", ptr(t) if t is not None else None, code, t.stride(0) * esz if t is not None else 0,
+                H, W, ptr(tables), ptr(dx), ptr(dy), int(terrain), float(zfactor), ptr(out), out.stride(0) * esz,
+                ptr(stats), ptr(scratch), size)
         if index_out_of_range(stats.cpu().numpy()):
             raise IndexError("index out of bounds for the permutation table of size %d" % INDEX_LIMIT)
-    return out.cpu().numpy() if isinstance(data, np.ndarray) else like_container(out, data)
+    return to_container(out, data)
 
 
 def perlin(agg, freq=(1, 1), seed=5, name='perlin'):

@@ -5,14 +5,11 @@ row-major order.  The reference's GDAL-style sweep (proximity.py:261-398) passes
 its neighbours and can miss the nearest one; where it finds it, the outputs are equal (DESIGN.md section 4.7).
 The distance, allocation and direction values follow the reference's formulas and float32 roundings.
 """
-import ctypes
-
 import numpy as np
 
-from . import _lib
 from ._xr import DataArray
 from .dataset_support import supports_dataset
-from .utils import device_2d, is_dask_array, is_device_array, like_container, stream_ptr
+from .utils import call_on, coord, device_cells, device_scratch, pitch, ptr, to_container
 
 EUCLIDEAN = 0
 GREAT_CIRCLE = 1
@@ -23,11 +20,6 @@ ALLOCATION = 1
 DIRECTION = 2
 
 DISTANCE_METRICS = {"EUCLIDEAN": EUCLIDEAN, "GREAT_CIRCLE": GREAT_CIRCLE, "MANHATTAN": MANHATTAN}
-
-# numpy cell types the kernels read as they are, and the type each other one is widened to without changing a value
-_DTYPE_CODES = {np.dtype(k): v for k, v in _lib.DTYPES.items()}
-_WIDEN = {np.dtype(np.bool_): np.int16, np.dtype(np.int8): np.int16, np.dtype(np.uint8): np.int16,
-          np.dtype(np.uint32): np.int64, np.dtype(np.uint64): np.int64, np.dtype(np.float16): np.float32}
 
 
 def euclidean_distance(x1: float, x2: float, y1: float, y2: float) -> float:
@@ -72,35 +64,6 @@ def _monotone(v, name):
             "proximity needs the 1-D coordinate %r to be finite and strictly ascending or descending" % name)
 
 
-def _coord(raster, name):
-    c = raster[name]
-    return np.ascontiguousarray(getattr(c, "data", c), dtype=np.float64)
-
-
-def _cells(data):
-    """The raster as a 2-D CUDA tensor of one of the library's cell types, and that type's code."""
-    import torch
-    if isinstance(data, np.ndarray):
-        widen = _WIDEN.get(data.dtype)
-        if data.dtype == np.uint64 and data.size and data.max() > np.iinfo(np.int64).max:
-            raise ValueError("uint64 cells above 2**63 - 1 are not supported")
-        if widen is not None:
-            data = data.astype(widen)
-        if data.dtype not in _DTYPE_CODES:
-            raise TypeError("unsupported cell type %s" % data.dtype)
-        t = device_2d(data)
-    else:
-        t = device_2d(data)
-        widen = {torch.bool: torch.int16, torch.int8: torch.int16, torch.uint8: torch.int16,
-                 torch.uint32: torch.int64, torch.float16: torch.float32, torch.bfloat16: torch.float32}
-        if t.dtype in widen:
-            t = t.to(widen[t.dtype])
-    code = _lib.DTYPES.get(str(t.dtype).replace("torch.", ""))
-    if code is None:
-        raise TypeError("unsupported cell type %s" % t.dtype)
-    return t, code
-
-
 def _process(raster, x, y, target_values, max_distance, distance_metric, process_mode, band_rows=0):
     """The transform behind proximity / allocation / direction (proximity.py:401-647): float32 raster of the
     distance, the nearest target's value or the direction to it.  `band_rows` (0: the library's choice) only
@@ -111,17 +74,12 @@ def _process(raster, x, y, target_values, max_distance, distance_metric, process
     metric = DISTANCE_METRICS.get(distance_metric, EUCLIDEAN)
     if max_distance is None:
         max_distance = np.inf
-    data = raster.data
-    if is_dask_array(data):
-        raise NotImplementedError("proximity: Dask arrays are not supported by the GPU backend")
-    if not (isinstance(data, np.ndarray) or is_device_array(data)):
-        raise TypeError("Unsupported Array Type: {}".format(type(data)))
-    xs, ys = _coord(raster, x), _coord(raster, y)
+    xs, ys = (np.ascontiguousarray(coord(raster, d), dtype=np.float64) for d in (x, y))
     _monotone(xs, x)
     _monotone(ys, y)
     if metric == GREAT_CIRCLE and xs.size and ys.size:
         _check_lon_lat(xs.min(), xs.max(), ys.min(), ys.max())
-    t, code = _cells(data)
+    t, code = device_cells(raster.data, "proximity", "widen")
     H, W = t.shape
     if (len(xs), len(ys)) != (W, H):
         raise ValueError("coordinate lengths (%d, %d) do not match the raster's shape %s" % (len(ys), len(xs), (H, W)))
@@ -134,21 +92,15 @@ def _process(raster, x, y, target_values, max_distance, distance_metric, process
             vals = vals[~np.isnan(vals)]
             # never a NULL list (the default rule), also when no value can match
             targets = torch.as_tensor(np.append(vals, 0.0), device=t.device)[:vals.size]
-        need = ctypes.c_int64()
-        _lib.call("xrs_proximity_scratch_bytes", H, W, int(band_rows), ctypes.byref(need))
-        scratch = torch.empty(need.value, dtype=torch.uint8, device=t.device)
+        scratch, size = device_scratch("xrs_proximity_scratch_bytes", H, W, int(band_rows), device=t.device,
+                                       what="proximity")
         xt = torch.as_tensor(xs, device=t.device)
         yt = torch.as_tensor(ys, device=t.device)
-        with torch.cuda.device(t.device):
-            _lib.call("xrs_proximity", ctypes.c_void_p(t.data_ptr()), code, t.stride(0) * t.element_size(), H, W,
-                      ctypes.c_void_p(xt.data_ptr()), ctypes.c_void_p(yt.data_ptr()),
-                      None if targets is None else ctypes.c_void_p(targets.untyped_storage().data_ptr()),
-                      0 if targets is None else vals.size, float(max_distance), metric, int(process_mode),
-                      ctypes.c_void_p(out.data_ptr()), out.stride(0) * 4, ctypes.c_void_p(scratch.data_ptr()),
-                      need.value, int(band_rows), stream_ptr(t))
-    if isinstance(data, np.ndarray):
-        return out.cpu().numpy()
-    return like_container(out, data)
+        call_on(t, "xrs_proximity", ptr(t), code, pitch(t), H, W, ptr(xt), ptr(yt),
+                None if targets is None else ptr(targets.untyped_storage()),
+                0 if targets is None else vals.size, float(max_distance), metric, int(process_mode), ptr(out),
+                pitch(out), ptr(scratch), size, int(band_rows))
+    return to_container(out, raster.data)
 
 
 def _wrap(result, raster):

@@ -175,9 +175,10 @@ def _dbl_array(vals):
 
 
 def device_2d(data, dtype=None):
-    """2-D CUDA tensor with unit inner stride, cast to `dtype` when given (like the reference's
-    `data.astype(cupy.float32)`, slope.py:150).  A numpy raster is cast on the host and uploaded; a
-    device array is viewed, and cast or copied only if needed."""
+    """2-D CUDA tensor with unit inner stride and rows at least a row apart, cast to `dtype` when given (like the
+    reference's `data.astype(cupy.float32)`, slope.py:150).  A numpy raster is cast on the host and uploaded; a
+    device array is viewed, and cast or copied only if needed (a broadcast raster, whose rows share memory, is
+    copied)."""
     if isinstance(data, np.ndarray):
         if data.ndim != 2:
             raise ValueError("expected a 2-D raster, got %d-D" % data.ndim)
@@ -188,9 +189,97 @@ def device_2d(data, dtype=None):
         raise ValueError("expected a 2-D raster, got %d-D" % t.dim())
     if dtype is not None and t.dtype != dtype:
         t = t.to(dtype)
-    if t.numel() and t.stride(1) != 1:
-        t = t.contiguous()
+    if t.numel() and (t.stride(1) != 1 or t.stride(0) < t.shape[1]):
+        t = t.clone(memory_format=torch.contiguous_format)   # contiguous() keeps the strides of a 1-row view
     return t
+
+
+# How each family of device entry points takes a raster's cells (xrs_b200.h names the cell sets):
+#   widen: proximity, viewshed, a_star_search and classify read the raster set; other integer and float types are
+#          widened to one of it without changing a value;
+#   as-is: regions, trim and crop read every zonal cell type as it is;
+#   float: perlin and generate_terrain take float32 and float64 only.
+# Each policy: (codes of the cell types read, widening, error for another type, its message).
+_WIDEN = {"bool": "int16", "int8": "int16", "uint8": "int16", "uint32": "int64", "uint64": "int64",
+          "float16": "float32", "bfloat16": "float32"}
+CELL_POLICIES = {
+    "widen": (_lib.DTYPES, _WIDEN, TypeError, "%s: unsupported cell type %s"),
+    "as-is": (_lib.ZONAL_CELLS, {}, NotImplementedError, "%s: %s rasters are not supported (nor by the reference)"),
+    "float": ({k: _lib.DTYPES[k] for k in ("float32", "float64")}, {}, TypeError,
+              "%s takes float32 or float64 cells, not %s"),
+}
+
+
+def raster_cells(data, what, policy):
+    """A numpy or device 2-D raster checked against CELL_POLICIES[policy], as the numpy array or CUDA tensor of the
+    cells the entry point reads, and their code.  Nothing is uploaded."""
+    if is_dask_array(data):
+        raise NotImplementedError("%s: Dask arrays are not supported by the GPU backend" % what)
+    if isinstance(data, np.ndarray):
+        a = data
+    elif is_device_array(data):
+        a = as_device_tensor(data)
+    else:
+        raise TypeError("Unsupported raster array type: {}".format(type(data)))
+    if a.ndim != 2:
+        raise ValueError("%s needs a 2-D raster, got %d-D" % (what, a.ndim))
+    codes, widen, error, message = CELL_POLICIES[policy]
+    name = str(a.dtype).replace("torch.", "")
+    host = isinstance(a, np.ndarray)
+    if name == "uint64" and widen.get(name) == "int64":
+        # uint64 cells below 2**63 are their own int64 view; the others are the negative ones of it
+        a, name = a.view(np.int64 if host else torch.int64), "int64"
+        if bool((a < 0).any()):
+            raise ValueError("%s: uint64 cells above 2**63 - 1 are not supported" % what)
+    elif name in widen:
+        name = widen[name]
+        a = a.astype(name) if host else a.to(getattr(torch, name))
+    if name not in codes:
+        raise error(message % (what, name))
+    return a, codes[name]
+
+
+def device_cells(data, what, policy):
+    """raster_cells on the device: (a 2-D CUDA tensor as device_2d gives it, the cells' code)."""
+    a, code = raster_cells(data, what, policy)
+    return device_2d(a), code
+
+
+def device_scratch(query, *query_args, device, what):
+    """(a device buffer of the bytes `query(*query_args)` asks for, that size).  MemoryError when the device
+    cannot allocate it."""
+    need = ctypes.c_int64()
+    _lib.call(query, *query_args, ctypes.byref(need))
+    try:
+        return torch.empty(max(1, need.value), dtype=torch.uint8, device=device), need.value
+    except torch.OutOfMemoryError as e:
+        raise MemoryError("%s needs %d bytes of device scratch" % (what, need.value)) from e
+
+
+def ptr(t):
+    return ctypes.c_void_p(t.data_ptr())
+
+
+def pitch(t):
+    """Bytes between the rows of a 2-D tensor."""
+    return t.stride(0) * t.element_size()
+
+
+def call_on(t, name, *args):
+    """The entry point `name(*args, stream)` on tensor t's device, on torch's current stream there."""
+    with torch.cuda.device(t.device):
+        _lib.call(name, *args, stream_ptr(t))
+
+
+def to_container(out, data):
+    """A device result `out` in the container of the raster `data`: numpy for numpy, else like_container."""
+    return out.cpu().numpy() if isinstance(data, np.ndarray) else like_container(out, data)
+
+
+def coord(raster, name):
+    """raster[name] as a numpy array (the integer index when the raster has no such coordinate)."""
+    c = raster[name]
+    return np.asarray(getattr(c, "data", c))
 
 
 def run_stencil_device(fn_name, data, *args, dtype=None):

@@ -8,22 +8,13 @@ One deviation: the reference raises ValueError("node not found") when a NaN cell
 of the observer.  This implementation returns the well-defined result instead: NaN cells are -1 (invisible) and
 never block the view of other cells, as everywhere else in the raster.
 """
-import ctypes
-
 import numpy as np
 
-from . import _lib
 from ._xr import DataArray
-from .proximity import _cells
-from .utils import is_dask_array, is_device_array, like_container, stream_ptr
+from .utils import call_on, coord, device_2d, device_scratch, pitch, ptr, raster_cells, to_container
 
 OBS_ELEV = 0
 TARGET_ELEV = 0
-
-
-def _coord(raster, name):
-    c = raster[name]
-    return np.ascontiguousarray(getattr(c, "data", c))
 
 
 def _nearest(coords, v):
@@ -59,33 +50,20 @@ def viewshed(raster, x, y, observer_elev=OBS_ELEV, target_elev=TARGET_ELEV):
     raises when one lies in the observer's row east of it)."""
     import torch
     data = raster.data
-    if is_dask_array(data):
-        raise NotImplementedError("viewshed: Dask arrays are not supported by the GPU backend")
-    if not (isinstance(data, np.ndarray) or is_device_array(data)):
-        raise TypeError("Unsupported raster array type: {}".format(type(data)))
-    xs, ys = _coord(raster, "x"), _coord(raster, "y")
-    if (len(xs), len(ys)) != tuple(data.shape[::-1]):
+    cells, code = raster_cells(data, "viewshed", "widen")
+    xs, ys = coord(raster, "x"), coord(raster, "y")
+    if (len(xs), len(ys)) != tuple(cells.shape[::-1]):
         raise ValueError("coordinate lengths (%d, %d) do not match the raster's shape %s"
-                         % (len(ys), len(xs), tuple(data.shape)))
+                         % (len(ys), len(xs), tuple(cells.shape)))
     if isinstance(data, np.ndarray):
         view = _view(xs, ys, x, y, lambda r, c: data[r, c], observer_elev, target_elev)
-        t, code = _cells(data)
     else:
-        t, code = _cells(data)
-        view = _view(xs, ys, x, y, lambda r, c: t[r, c].cpu().numpy()[()], observer_elev, target_elev)
+        view = _view(xs, ys, x, y, lambda r, c: cells[r, c].cpu().numpy()[()], observer_elev, target_elev)
+    t = device_2d(cells)
     vr, vc, vp_elev, target, ew_res, ns_res = view
     H, W = t.shape
-    need = ctypes.c_int64()
-    _lib.call("xrs_viewshed_scratch_bytes", H, W, ctypes.byref(need))
-    try:
-        scratch = torch.empty(need.value, dtype=torch.uint8, device=t.device)
-    except torch.OutOfMemoryError as e:
-        raise MemoryError("viewshed needs %d bytes of device scratch for a %d x %d raster"
-                          % (need.value, H, W)) from e
+    scratch, size = device_scratch("xrs_viewshed_scratch_bytes", H, W, device=t.device, what="viewshed")
     out = torch.empty((H, W), dtype=torch.float64, device=t.device)
-    with torch.cuda.device(t.device):
-        _lib.call("xrs_viewshed", ctypes.c_void_p(t.data_ptr()), code, t.stride(0) * t.element_size(), H, W, vr, vc,
-                  vp_elev, target, ew_res, ns_res, ctypes.c_void_p(out.data_ptr()), out.stride(0) * 8,
-                  ctypes.c_void_p(scratch.data_ptr()), need.value, stream_ptr(t))
-    result = out.cpu().numpy() if isinstance(data, np.ndarray) else like_container(out, data)
-    return DataArray(result, coords=raster.coords, dims=raster.dims, attrs=raster.attrs)
+    call_on(t, "xrs_viewshed", ptr(t), code, pitch(t), H, W, vr, vc, vp_elev, target, ew_res,
+            ns_res, ptr(out), pitch(out), ptr(scratch), size)
+    return DataArray(to_container(out, data), coords=raster.coords, dims=raster.dims, attrs=raster.attrs)

@@ -8,7 +8,6 @@ like the reference: zonal.py:640-642) run per zone on the zone's valid values, g
 by one sort.  With `comm` (a torch.distributed process group) the partials of row-striped rasters
 are combined with AllReduce before finalisation.
 """
-import ctypes
 import math
 
 import numpy as np
@@ -16,14 +15,10 @@ import pandas as pd
 
 from . import _lib
 from ._xr import DataArray, Dataset
-from .utils import (ArrayTypeFunctionMapping, as_device_tensor, is_dask_array, is_device_array, like_container,
-                    stream_ptr, validate_arrays)
+from .utils import (ArrayTypeFunctionMapping, as_device_tensor, call_on, device_cells, device_scratch, like_container,
+                    pitch, ptr, stream_ptr, to_container, validate_arrays)
 
 _DEFAULT_STATS = ("mean", "max", "min", "sum", "std", "var", "count", "majority")
-
-
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr())
 
 
 def _device_tensor(a):
@@ -123,11 +118,11 @@ def _table_pass(entry, zones_t, values_t, nodata_values, table_args, keys, acc, 
     packed = torch.empty(_HDR + 6 * _MAX_OUT, dtype=torch.float64, device=values_t.device)
     flags = torch.empty(3, dtype=torch.int32, device=values_t.device)
     with torch.cuda.device(values_t.device):
-        _lib.call(entry, _ptr(values_t), dt(values_t), _ptr(zones_t), dt(zones_t), values_t.numel(),
+        _lib.call(entry, ptr(values_t), dt(values_t), ptr(zones_t), dt(zones_t), values_t.numel(),
                   int(values_t.shape[-1]) if values_t.dim() else 1,
                   0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
-                  *(_ptr(a) if torch.is_tensor(a) else a for a in table_args), *(_ptr(r) for r in acc),
-                  keys.numel(), _ptr(packed), _MAX_OUT, _ptr(flags), stream_ptr(values_t))
+                  *(ptr(a) if torch.is_tensor(a) else a for a in table_args), *(ptr(r) for r in acc),
+                  keys.numel(), ptr(packed), _MAX_OUT, ptr(flags), stream_ptr(values_t))
     host = packed.cpu().numpy()                    # the one synchronising copy
     n_used, overflow, pivot, sentinel = int(host[0]), int(host[1]), float(host[2]), int(host[3])
     if overflow:
@@ -279,9 +274,9 @@ def pair_counts(zones_t, values_t, nodata_values=None, comm=None, cap=None, max_
         count = torch.empty(cap, dtype=torch.int64, device=dev)
         ovf = torch.empty(1, dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
-            _lib.call("xrs_zonal_pair_count", _ptr(vf), _ptr(zi), vf.numel(), int(vf.shape[-1]) if vf.dim() else 1,
+            _lib.call("xrs_zonal_pair_count", ptr(vf), ptr(zi), vf.numel(), int(vf.shape[-1]) if vf.dim() else 1,
                       0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
-                      _ptr(keys), _ptr(count), cap, _ptr(ovf), stream_ptr(vf))
+                      ptr(keys), ptr(count), cap, ptr(ovf), stream_ptr(vf))
         if int(ovf.item()) == 0:
             break
         if cap >= max_cap:
@@ -804,33 +799,6 @@ def crosstab(zones, values, zone_ids=None, cat_ids=None, layer=None, agg="count"
 
 
 # ----------------------------------------------------------------------------- regions, trim, crop
-def _raster_cells(data, what):
-    """The raster as a 2-D CUDA tensor with unit column stride, and its cell type's code for zonal_regions.cu."""
-    import torch
-    if is_dask_array(data):
-        raise NotImplementedError("%s: Dask arrays are not supported by the GPU backend" % what)
-    if isinstance(data, np.ndarray):
-        if data.dtype == np.float16:
-            raise NotImplementedError("%s: float16 rasters are not supported (nor by the reference)" % what)
-        t = torch.from_numpy(np.ascontiguousarray(data)).cuda()
-    elif is_device_array(data):
-        t = as_device_tensor(data)
-    else:
-        raise TypeError("Unsupported raster array type: {}".format(type(data)))
-    if t.ndim != 2:
-        raise ValueError("%s needs a 2-D raster, got %d dimensions" % (what, t.ndim))
-    code = _lib.ZONAL_CELLS.get(str(t.dtype).replace("torch.", ""))
-    if code is None:
-        raise NotImplementedError("%s: %s rasters are not supported (nor by the reference)" % (what, t.dtype))
-    if t.stride(1) != 1 or t.stride(0) < t.shape[1]:
-        t = t.contiguous()
-    return t, code
-
-
-def _pitch(t):
-    return max(t.stride(0), t.shape[1]) * t.element_size()
-
-
 def regions(raster, neighborhood=4, name="regions"):
     """Number the connected regions of cells with close values (zonal.py:1552-1640 of the reference).
 
@@ -843,22 +811,14 @@ def regions(raster, neighborhood=4, name="regions"):
     if neighborhood not in (4, 8):
         raise ValueError("`neighborhood` value must be either 4 or 8)")
     data = raster.data
-    t, code = _raster_cells(data, "regions")
+    t, code = device_cells(data, "regions", "as-is")
     H, W = t.shape
     out = torch.empty((H, W), dtype=t.dtype, device=t.device)
     if H and W:
-        need = ctypes.c_int64()
-        _lib.call("xrs_zonal_regions_scratch_bytes", H, W, ctypes.byref(need))
-        try:
-            scratch = torch.empty(need.value, dtype=torch.uint8, device=t.device)
-        except torch.OutOfMemoryError as e:
-            raise MemoryError("regions needs %d bytes of device scratch for a %d x %d raster"
-                              % (need.value, H, W)) from e
-        with torch.cuda.device(t.device):
-            _lib.call("xrs_zonal_regions", _ptr(t), code, _pitch(t), H, W, neighborhood, _ptr(out),
-                      W * out.element_size(), _ptr(scratch), need.value, stream_ptr(t))
-    result = out.cpu().numpy() if isinstance(data, np.ndarray) else like_container(out, data)
-    return DataArray(result, name=name, dims=raster.dims, coords=raster.coords, attrs=raster.attrs)
+        scratch, size = device_scratch("xrs_zonal_regions_scratch_bytes", H, W, device=t.device, what="regions")
+        call_on(t, "xrs_zonal_regions", ptr(t), code, pitch(t), H, W, neighborhood, ptr(out), pitch(out),
+                ptr(scratch), size)
+    return DataArray(to_container(out, data), name=name, dims=raster.dims, coords=raster.coords, attrs=raster.attrs)
 
 
 def _bounds(data, values, mode, what):
@@ -866,7 +826,7 @@ def _bounds(data, values, mode, what):
     last rows and columns holding a cell that equals none of `values` (trim) or one of them (crop), and
     (rows - 1, 0, cols - 1, 0) when no cell does."""
     import torch
-    t, code = _raster_cells(data, what)
+    t, code = device_cells(data, what, "as-is")
     H, W = t.shape
     vals = list(values)
     # numba types a list of ints as int64 and compares integer cells with them exactly; any float makes it float64
@@ -874,9 +834,8 @@ def _bounds(data, values, mode, what):
     dv = torch.tensor([float(v) for v in vals], dtype=torch.float64, device=t.device)
     iv = torch.tensor([int(v) for v in vals], dtype=torch.int64, device=t.device) if ints and vals else None
     out4 = torch.empty(4, dtype=torch.int64, device=t.device)
-    with torch.cuda.device(t.device):
-        _lib.call("xrs_zonal_bounds", _ptr(t), code, _pitch(t), H, W, mode, _ptr(dv) if vals else None,
-                  _ptr(iv) if iv is not None else None, len(vals), _ptr(out4), stream_ptr(t))
+    call_on(t, "xrs_zonal_bounds", ptr(t), code, pitch(t), H, W, mode, ptr(dv) if vals else None,
+            ptr(iv) if iv is not None else None, len(vals), ptr(out4))
     top, bottom, left, right = out4.cpu().tolist()
     if bottom < 0:
         return max(H - 1, 0), 0, max(W - 1, 0), 0
