@@ -331,7 +331,7 @@ __device__ __forceinline__ float atan_sqrt_deg(float p) {
     return fmaf(a, atan_poly01<1>(a * a), off);
 }
 
-// Compass aspect from the exact Horn sums X = 8 dz_dx, Y = 8 dz_dy (aspect.py:74-88):
+// Compass aspect from the Horn sums X = 8 dz_dx, Y = 8 dz_dy (aspect.py:74-88):
 // the reference's (90 - atan2(Y, -X) deg) folded to [0, 360) is atan2(u, v) with u = -X, v = Y,
 // folded to [0, 360).  One octant reduction (ratio t of the smaller to the larger magnitude,
 // one MUFU.RCP, degree-7 polynomial already scaled to degrees), then compass = K + sigma*atan(t)
@@ -339,7 +339,9 @@ __device__ __forceinline__ float atan_sqrt_deg(float p) {
 // so the tail is one FMA:  ts * poly(ts^2) + K.  Evaluating the compass angle directly keeps full
 // relative accuracy near 0 degrees, where `90 - theta` would cancel.  Flat cells (both sums zero)
 // give -1; NaN propagates (selects, not fmin/fmax, pick the operands; the flat test is NaN-safe:
-// a NaN sum next to a zero sum is NaN, like atan2(0, NaN) in the reference).
+// a NaN sum next to a zero sum is NaN, like atan2(0, NaN) in the reference).  The reciprocal is
+// rcp.approx.ftz: it needs normal max(|u|, |v|) <= 2^125 (its result is then a normal float); the
+// 3x3 aspect scales larger pairs first (surface_ops.cuh, compass_uv4).
 struct CompassPre {
     float ts, K;
     bool flat;

@@ -2,8 +2,11 @@
 //
 // Numerics follow the reference's *CPU* kernels, which do the Horn sums in float64 because
 // Numba promotes `2 * f32` (SURVEY.md section 0 fact 5): the column differences / weighted row
-// sums are formed in f64 (they are EXACT there for any realistic raster: sums of <= 8
-// float32 values), so re-associating them row by row changes nothing; the transcendental
+// sums are formed in f64 (sums of <= 8 float32 values: exact whenever the window's cells lie
+// within a factor 2^26 of each other), so re-associating them row by row changes nothing there.
+// Where a window mixes terrain with a fill beyond that range (a row of -FLT_MAX), the reference's
+// column-by-column X rounds the terrain away and these row differences do not: a documented
+// deviation (DESIGN.md 4.1, "Fill values"); the transcendental
 // tail (sqrt / atan / atan2) is evaluated in f32 on the correctly-rounded f64 intermediate,
 // which keeps the result within ~3e-7 relative of the oracle (bar: 1e-5).
 #pragma once
@@ -89,9 +92,49 @@ using SlopeOp = SlopeOpT<false>;
 using SlopeSqOp = SlopeOpT<true>;
 
 // ------------------------------------------------------------------ aspect (aspect.py:56-90)
-// X = 8*dz_dx, Y = 8*dz_dy, exact in f64; rounding them to f32 (6e-8) before the octant
-// reduction is far inside the 1e-5 bar, and (float)X == 0 iff X == 0 for any raster whose
-// cells are not denormal, so the flat (-1) mask is the reference's bit for bit.
+// X = 8*dz_dx, Y = 8*dz_dy in f64; rounding them to f32 (6e-8) before the octant reduction is
+// far inside the 1e-5 bar, and (float)X == 0 iff X == 0 (X is 0 or at least 2^-149, which f32
+// keeps) for any raster whose cells are not denormal, so the flat (-1) mask is the reference's bit
+// for bit.  Denormal cells are not served: compass_pre's ftz reciprocal flushes a denormal sum.
+//
+// compass_uv4 gives compass_deg its (u, v) = (-X, Y) in f32.  Only their ratio and signs matter.
+// Next to a fill value such as -FLT_MAX the larger sum exceeds 2^125, where compass_pre's
+// reciprocal would flush to zero, or FLT_MAX, where the conversion would give inf; such a pair is
+// scaled by 2^-8 in f64 first (exact, and the flat test cannot change: the pair is far from 0).
+// An infinite sum (next to an infinite cell) counts as +-1 and a finite one as +-0, which is what
+// the reference's float64 atan2 gives for them.
+// compass_uv4 rounds the four cells of a lane and returns the largest |u|, |v| (7 FMNMX); only when
+// it exceeds 2^125 (one compare and one branch per lane) does compass_wide4 rewrite the wide pairs,
+// out of line so that the hot loop keeps its registers.
+__device__ __noinline__ float2 compass_uv_wide(double X, double Y, float u, float v) {
+    if (!(fmaxf(fabsf(u), fabsf(v)) > 0x1p125f)) return make_float2(u, v);   // fmaxf drops a NaN: it propagates
+    const bool ix = isinf(X), iy = isinf(Y);
+    if (ix || iy)
+        return make_float2(ix ? copysignf(1.0f, u) : (float)(X * -0.0),   // X * 0 keeps a NaN
+                           iy ? copysignf(1.0f, v) : (float)(Y * 0.0));
+    return make_float2((float)(X * -0x1p-8), (float)(Y * 0x1p-8));
+}
+__device__ __forceinline__ float compass_uv4(const double (&X)[4], const double (&Y)[4], float (&u)[4],
+                                             float (&v)[4]) {
+    float m = 0.0f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        u[i] = (float)(-X[i]);
+        v[i] = (float)Y[i];
+        m = fmaxf(m, fmaxf(fabsf(u[i]), fabsf(v[i])));
+    }
+    return m;
+}
+constexpr float kCompassWide = 0x1p125f;
+__device__ __forceinline__ void compass_wide4(const double (&X)[4], const double (&Y)[4], float (&u)[4],
+                                              float (&v)[4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float2 w = compass_uv_wide(X[i], Y[i], u[i], v[i]);
+        u[i] = w.x;
+        v[i] = w.y;
+    }
+}
 __device__ __forceinline__ void aspect_tail4(const float (&u)[4], const float (&v)[4], float (&out)[4]) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) out[i] = compass_deg(u[i], v[i]);
@@ -111,13 +154,13 @@ struct AspectOp {
     __device__ __forceinline__ void step(const Row6<float> &row, Vec4<float> (&out)[1]) {
         const HornRow n = horn_row(row);
         float u[4], v[4];
+        double X[4], Y[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            const double X = fma(2.0, m1.D[i], m2.D[i]) + n.D[i];
-            const double Y = n.S[i] - m2.S[i];  // a,b,c = row y-1 here (aspect.py:65-72)
-            u[i] = (float)(-X);
-            v[i] = (float)Y;
+            X[i] = fma(2.0, m1.D[i], m2.D[i]) + n.D[i];
+            Y[i] = n.S[i] - m2.S[i];  // a,b,c = row y-1 here (aspect.py:65-72)
         }
+        if (compass_uv4(X, Y, u, v) > kCompassWide) compass_wide4(X, Y, u, v);   // rare: next to fills
         aspect_tail4(u, v, out[0].v);
         m2 = m1;
         m1 = n;
@@ -199,20 +242,48 @@ struct HillshadeOp {
         for (int i = 0; i < 4; ++i) n2[i] = 0.f, r1.c[i] = 0.f;
         r1.l = r1.r = 0.f;
     }
-    static __device__ __forceinline__ float eval(float gx2, float gy2, const Params &p) {
-        // gx2 = 2*d/drow, gy2 = 2*d/dcol
-        const float q = fmaf(gx2, gx2, gy2 * gy2);
-        const float rinv = rsqrt_approx(fmaf(0.25f, q, 1.0f));
-        const float num = fmaf(p.cy, gy2, fmaf(-p.cx, gx2, p.s0));
-        return fmaf(0.5f * num, rinv, 0.5f);
+    // Where q = gx2^2 + gy2^2 overflows f32 (a fill value such as -FLT_MAX next to terrain, |grad| > 9e18) the
+    // closed form would give 0.5 or NaN.  Its limit for a large gradient, 0.5 + (cy gy2 - cx gx2) / |(gx2, gy2)|,
+    // is the reference's value there: its f32 x*x + y*y overflows as well (slope 0) and cos(A - aspect) is the
+    // same direction cosine.  Only the direction matters, so the pair is scaled by 2^-100 (it is then below
+    // 2^28, above 2^-38); an infinite component (an infinite cell) counts as +-1 against 0, as in atan2.
+    static __device__ __noinline__ float steep(float gx2, float gy2, const Params &p) {
+        const bool ix = isinf(gx2), iy = isinf(gy2);
+        const float s = (ix || iy) ? 0.0f : 0x1p-100f;
+        const float x = ix ? copysignf(1.0f, gx2) : gx2 * s;
+        const float y = iy ? copysignf(1.0f, gy2) : gy2 * s;
+        return fmaf(fmaf(p.cy, y, -p.cx * x), rsqrt_approx(fmaf(x, x, y * y)), 0.5f);
+    }
+    // the four cells of a lane (gx2 = 2*d/drow, gy2 = 2*d/dcol, q their squared norm); returns the largest q,
+    // which is inf where steep4 has to rewrite a cell (3 FMNMX)
+    static __device__ __forceinline__ float eval4(const float (&gx2)[4], const float (&gy2)[4], const Params &p,
+                                                  float (&q)[4], float (&out)[4]) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            q[i] = fmaf(gx2[i], gx2[i], gy2[i] * gy2[i]);
+            const float rinv = rsqrt_approx(fmaf(0.25f, q[i], 1.0f));
+            const float num = fmaf(p.cy, gy2[i], fmaf(-p.cx, gx2[i], p.s0));
+            out[i] = fmaf(0.5f * num, rinv, 0.5f);
+        }
+        return fmaxf(fmaxf(q[0], q[1]), fmaxf(q[2], q[3]));
+    }
+    static __device__ __forceinline__ void steep4(const float (&gx2)[4], const float (&gy2)[4], const Params &p,
+                                                  const float (&q)[4], float (&out)[4]) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+            if (q[i] == INFINITY) out[i] = steep(gx2[i], gy2[i], p);
     }
     __device__ __forceinline__ void step(const Row6<float> &row, Vec4<float> (&out)[1]) {
+        float gx2[4], gy2[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const float e = (i == 3) ? r1.r : r1.c[i + 1];
             const float w = (i == 0) ? r1.l : r1.c[i - 1];
-            out[0].v[i] = eval(row.c[i] - n2[i], e - w, p);
+            gx2[i] = row.c[i] - n2[i];
+            gy2[i] = e - w;
         }
+        float q[4];
+        if (eval4(gx2, gy2, p, q, out[0].v) == INFINITY) steep4(gx2, gy2, p, q, out[0].v);   // rare: next to fills
 #pragma unroll
         for (int i = 0; i < 4; ++i) n2[i] = r1.c[i];
         r1 = row;
@@ -247,18 +318,26 @@ template <bool SQUARE> struct SuiteOpT {
     }
     __device__ __forceinline__ void step(const Row6<float> &row, Vec4<float> (&out)[4]) {
         const HornRow n = horn_row(row);
-        float q[4], u[4], v[4];
+        float q[4], u[4], v[4], gx2[4], gy2[4];
+        double X[4], Y[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            const double X = fma(2.0, m1.D[i], m2.D[i]) + n.D[i];
+            X[i] = fma(2.0, m1.D[i], m2.D[i]) + n.D[i];
             const double Ys = m2.S[i] - n.S[i];
-            q[i] = slope_q<SQUARE>(X, Ys, p.slope);
-            u[i] = (float)(-X);
-            v[i] = (float)(-Ys);
+            q[i] = slope_q<SQUARE>(X[i], Ys, p.slope);
+            Y[i] = -Ys;
             const float e = (i == 3) ? r1.r : r1.c[i + 1];
             const float w = (i == 0) ? r1.l : r1.c[i - 1];
             out[2].v[i] = CurvatureOp::eval(row.c[i] + n2[i], e + w, r1.c[i], p.curv.k);
-            out[3].v[i] = HillshadeOp::eval(row.c[i] - n2[i], e - w, p.hill);
+            gx2[i] = row.c[i] - n2[i];
+            gy2[i] = e - w;
+        }
+        float qh[4];
+        const float m = compass_uv4(X, Y, u, v);
+        const float qmax = HillshadeOp::eval4(gx2, gy2, p.hill, qh, out[3].v);
+        if (m > kCompassWide || qmax == INFINITY) {   // rare: next to fills; one test for aspect and hillshade
+            compass_wide4(X, Y, u, v);
+            HillshadeOp::steep4(gx2, gy2, p.hill, qh, out[3].v);
         }
         slope_tail4(q, p.slope.ky2, out[0].v);
         aspect_tail4(u, v, out[1].v);
@@ -317,22 +396,29 @@ struct Conv3Op {
 __constant__ double kRcp9[10] = {
     __builtin_nan(""), 1.0, 1.0 / 2, 1.0 / 3, 1.0 / 4, 1.0 / 5, 1.0 / 6, 1.0 / 7, 1.0 / 8, 1.0 / 9};
 __constant__ double kCnt9[10] = {0.0, 1.0, 2.0, 3.0, 4.0, 5.0, 6.0, 7.0, 8.0, 9.0};
+// A window of -0.0 cells sums to -0.0 here but to +0.0 in the reference, whose sum starts at +0.0:
+// the float32 quotient is fma(s, r, +0.0), the same bits as s * r except that -0.0 becomes +0.0 (the
+// float64 correction step below does the same).  An infinite sum (infinite cells, or float64 cells
+// beyond DBL_MAX / 9 in total) skips the correction step, whose residual would be inf - inf = NaN.
 // full window (9 valid cells): the same arithmetic with literal operands
 template <typename TOUT> __device__ __forceinline__ TOUT div_full9(double s) {
-    const double r9 = 1.0 / 9, q9 = s * r9;
-    if constexpr (sizeof(TOUT) == 4) return (float)q9;
-    else return fma(fma(-q9, 9.0, s), r9, q9);
+    const double r9 = 1.0 / 9;
+    if constexpr (sizeof(TOUT) == 4) {
+        return (float)fma(s, r9, 0.0);
+    } else {
+        const double q9 = s * r9, e = fma(-q9, 9.0, s);
+        return e == e ? fma(e, r9, q9) : q9;
+    }
 }
 template <typename TOUT> __device__ __forceinline__ TOUT div_count9(double s, int cnt) {
     const double r = kRcp9[cnt];
-    const double q = s * r;
     if constexpr (sizeof(TOUT) == 4) {
         // float32 result: s * (1/n) is within one f64 ulp of s / n, so the f32 rounding agrees
         // with the oracle except when s / n sits within 1e-16 of an f32 rounding boundary
-        return (float)q;
+        return (float)fma(s, r, 0.0);
     } else {
-        const double e = fma(-q, kCnt9[cnt], s);
-        return fma(e, r, q);
+        const double q = s * r, e = fma(-q, kCnt9[cnt], s);
+        return e == e ? fma(e, r, q) : q;
     }
 }
 
