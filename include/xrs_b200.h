@@ -164,8 +164,9 @@ int xrs_hotspots_classify_f32(const float *mean, int64_t n, double global_mean, 
  * Elementwise over n contiguous float32 cells; out is NaN where the denominator is 0. */
 /* multispectral._run_normalized_ratio_cupy (:862) -- ndvi, nbr, nbr2, ndmi */
 int xrs_normalized_ratio_f32(const float *a, const float *b, float *out, int64_t n, xrs_stream_t s);
-/* multispectral._savi_cupy (:912) */
-int xrs_savi_f32(const float *nir, const float *red, double soil_factor, float *out, int64_t n,
+/* multispectral._savi_cupy (:912); f32_sum != 0 sums nir + red + soil_factor in float32 (the soil factor's
+ * type decides, as in the reference's `_savi_cpu`), else in float64 */
+int xrs_savi_f32(const float *nir, const float *red, double soil_factor, int f32_sum, float *out, int64_t n,
                  xrs_stream_t s);
 /* multispectral._evi_cupy (:210) */
 int xrs_evi_f32(const float *nir, const float *red, const float *blue, double c1, double c2,

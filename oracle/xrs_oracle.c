@@ -287,8 +287,10 @@ XO_EXPORT void xo_normalized_ratio_f32(const float *a, const float *b, float *ou
         out[i] = (den == 0.0f) ? NAN : num / den;
     }
 }
-/* multispectral.py:876-890 `_savi_cpu`: numerator f32; soil_factor is a Python float, so
- * nir + red (f32) + soil_factor and the rest of the denominator are f64. */
+/* multispectral.py:876-890 `_savi_cpu` with a Python float soil_factor: numerator f32,
+ * nir + red (f32) + soil_factor and the rest of the denominator f64.  Numba sums
+ * nir + red + soil_factor in f32 instead when soil_factor is a float32, int8, int16, uint8 or
+ * bool; the device kernel follows that (its f32_sum flag), this oracle only the float64 sum. */
 XO_EXPORT void xo_savi_f32(const float *nir, const float *red, double soil, float *out,
                            int64_t n, int nthreads) {
 #pragma omp parallel for num_threads(nthreads) schedule(static)

@@ -50,7 +50,7 @@ def _declare(lib):
         "xrs_global_stats_f32": [P, I64, D, P, P],
         "xrs_hotspots_classify_f32": [P, I64, D, D, P, P],
         "xrs_normalized_ratio_f32": [P, P, P, I64, P],
-        "xrs_savi_f32": [P, P, D, P, I64, P],
+        "xrs_savi_f32": [P, P, D, I, P, I64, P],
         "xrs_evi_f32": [P, P, P, D, D, D, D, P, I64, P],
         "xrs_arvi_f32": [P, P, P, P, I64, P],
         "xrs_gci_f32": [P, P, P, I64, P],

@@ -12,11 +12,16 @@ struct NormRatio {  // multispectral.py:825-841 -- pure f32
         return den == 0.0f ? __int_as_float(0x7fc00000) : (a - b) / den;
     }
 };
-struct Savi {  // :876-890 -- numerator f32, denominator f64
+// :876-890 -- numerator f32; nir + red + L in the type Numba gives it, which follows L's type: f32 for a float32,
+// int8, int16, uint8 or bool L (f32_sum), f64 for a Python float or int and the wider NumPy types; the
+// product with 1 + L and the division are f64 either way.
+struct Savi {
     double L, onepL;
+    int f32_sum;
     __device__ __forceinline__ float operator()(float nir, float red, float) const {
         const float num = nir - red;
-        const double den = ((double)(nir + red) + L) * onepL;
+        const double soma = f32_sum ? (double)((nir + red) + (float)L) : (double)(nir + red) + L;
+        const double den = soma * onepL;
         return den != 0.0 ? (float)((double)num / den) : __int_as_float(0x7fc00000);
     }
 };
@@ -104,9 +109,9 @@ extern "C" {
 int xrs_normalized_ratio_f32(const float *a, const float *b, float *out, int64_t n, xrs_stream_t s) {
     return launch_band<2>(a, b, nullptr, out, n, NormRatio{}, s);
 }
-int xrs_savi_f32(const float *nir, const float *red, double soil_factor, float *out, int64_t n,
+int xrs_savi_f32(const float *nir, const float *red, double soil_factor, int f32_sum, float *out, int64_t n,
                  xrs_stream_t s) {
-    return launch_band<2>(nir, red, nullptr, out, n, Savi{soil_factor, 1.0 + soil_factor}, s);
+    return launch_band<2>(nir, red, nullptr, out, n, Savi{soil_factor, 1.0 + soil_factor, f32_sum}, s);
 }
 int xrs_evi_f32(const float *nir, const float *red, const float *blue, double c1, double c2,
                 double soil_factor, double gain, float *out, int64_t n, xrs_stream_t s) {

@@ -28,7 +28,8 @@ def _band_device(fn_name, bands, scalars=()):
     out = torch.empty(ts[0].shape, dtype=torch.float32, device=ts[0].device)
     n = out.numel()
     if n:
-        args = [ctypes.c_void_p(t.data_ptr()) for t in ts] + [float(s) for s in scalars]
+        args = [ctypes.c_void_p(t.data_ptr()) for t in ts]
+        args += [s if isinstance(s, ctypes.c_int) else float(s) for s in scalars]
         args += [ctypes.c_void_p(out.data_ptr()), n]
         with torch.cuda.device(out.device):
             _lib.call(fn_name, *args, stream_ptr(out))
@@ -54,6 +55,13 @@ def _mapper(fn_name):
 
 _NB = {"xrs_normalized_ratio_f32": 2, "xrs_savi_f32": 2, "xrs_evi_f32": 3, "xrs_arvi_f32": 3,
        "xrs_gci_f32": 2, "xrs_sipi_f32": 3, "xrs_ebbi_f32": 3}
+
+
+# Soil-factor types for which the reference's Numba kernel sums `nir + red + soil_factor` in float32; every
+# other accepted type (Python float and int, np.float64, np.int32, np.int64 and the unsigned types from uint16
+# up) gives a float64 sum.  NumPy's promotion rules do not give this table (float32 + uint16 is float32 in
+# NumPy, float64 in Numba), so it is pinned type by type by tests/golden/multispectral_edges.npz.
+_SAVI_F32_SUM = (np.float32, np.int8, np.int16, np.uint8, np.bool_, bool)
 
 
 def _wrap(out, like, name):
@@ -96,7 +104,8 @@ def savi(nir_agg, red_agg, soil_factor=1.0, name='savi'):
     validate_arrays(red_agg, nir_agg)
     if not -1.0 <= soil_factor <= 1.0:
         raise ValueError("soil factor must be between [-1.0, 1.0]")
-    out = _mapper("xrs_savi_f32")(red_agg)(nir_agg.data, red_agg.data, soil_factor)
+    f32_sum = ctypes.c_int(int(isinstance(soil_factor, _SAVI_F32_SUM)))
+    out = _mapper("xrs_savi_f32")(red_agg)(nir_agg.data, red_agg.data, soil_factor, f32_sum)
     return _wrap(out, nir_agg, name)
 
 
