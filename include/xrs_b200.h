@@ -455,6 +455,28 @@ int xrs_synth_terrain_f32(float *out, int64_t out_pitch, int64_t H, int64_t W,
                           int64_t row0, int64_t col0, uint64_t seed, float zmin, float zmax,
                           xrs_stream_t s);
 
+/* ------------------------------------------------------------------ local (local.cu)
+ * The reference's local.py, cell by cell over K layers.  `layers`: a HOST array of K {pointer, pitch in bytes,
+ * dtype} triples of int64, each layer a DEVICE raster of the zonal set (XRS_U64 cells below 2**63); `layers_dev`: a
+ * DEVICE buffer of 24 K bytes the entry point copies them to on `stream`.
+ * xrs_local_cells: op 0-12 (sum, mean, median, min, max, std, lesser / equal / greater frequency, lowest /
+ * highest position, popularity, rank; local_rule.cuh), ak the stack's array kind (0 float, 1 int, 2 bool).  The
+ * frequencies, popularity and rank read the ref raster `ref` (ref_f16: float16 cells carried as float32).  out:
+ * H x W int64 (a double's bits for float results; -1 for a NaN count or position); popularity and rank also write
+ * each cell's kind (0 float, 1 int, 2 bool) to `kinds`.  *flags (DEVICE, zeroed by the caller) gets the OR of the
+ * cells' flags: 1 NaN, 2 IndexError, 4 TypeError, 8 a float result, 16 an int result.
+ * xrs_local_combine: phase 0 fills the table in scratch (xrs_local_combine_scratch_bytes(H, W): 8 bytes per slot,
+ * a power of two at least twice the cells) with each distinct non-NaN tuple's first cell index, and sets flag 1
+ * for NaN cells; the caller then stores -1 - id in every occupied slot, reps[id] being that slot's first cell;
+ * phase 1 writes each cell's id + 1 (-1 for NaN) to out. */
+int xrs_local_cells(const int64_t *layers, int64_t K, void *layers_dev, int64_t H, int64_t W, int op, int ak,
+                    const void *ref, int64_t ref_pitch, int ref_dtype, int ref_f16, int64_t *out, int64_t out_pitch,
+                    uint8_t *kinds, int64_t kinds_pitch, unsigned *flags, void *stream);
+int xrs_local_combine_scratch_bytes(int64_t H, int64_t W, int64_t *bytes);
+int xrs_local_combine(const int64_t *layers, int64_t K, void *layers_dev, int64_t H, int64_t W, int phase,
+                      void *scratch, int64_t scratch_bytes, const int64_t *reps, int64_t *out, int64_t out_pitch,
+                      unsigned *flags, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,6 +14,7 @@ from .curvature import curvature  # noqa: F401
 from .focal import apply as focal_apply  # noqa: F401
 from .focal import focal_stats, hotspots, mean  # noqa: F401
 from .hillshade import hillshade  # noqa: F401
+from . import local  # noqa: F401
 from .proximity import allocation, direction, euclidean_distance, great_circle_distance  # noqa: F401
 from .proximity import manhattan_distance, proximity  # noqa: F401
 from .pathfinding import a_star_search  # noqa: F401

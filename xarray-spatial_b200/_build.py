@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libxrs_b200.so")
-SOURCES = ["lib_core.cu", "surface.cu", "multispectral.cu", "conv.cu", "box_stream.cu", "zonal_hash.cu", "hotspots.cu", "geodesic.cu", "proximity.cu", "viewshed.cu", "pathfinding.cu", "noise.cu", "classify.cu", "natural_breaks.cu", "zonal_regions.cu", "host.cu", "synth.cu"]
+SOURCES = ["lib_core.cu", "surface.cu", "multispectral.cu", "conv.cu", "box_stream.cu", "zonal_hash.cu", "hotspots.cu", "geodesic.cu", "proximity.cu", "viewshed.cu", "pathfinding.cu", "noise.cu", "classify.cu", "natural_breaks.cu", "zonal_regions.cu", "local.cu", "host.cu", "synth.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [
     "-O3", "-lineinfo", "-std=c++17",

@@ -87,6 +87,9 @@ def _declare(lib):
         "xrs_zonal_regions_scratch_bytes": [I64, I64, ctypes.POINTER(I64)],
         "xrs_zonal_regions": [P, I, I64, I64, I64, I, P, I64, P, I64, P],
         "xrs_zonal_bounds": [P, I, I64, I64, I64, I, P, P, I, P, P],
+        "xrs_local_cells": [P, I64, P, I64, I64, I, I, P, I64, I, I, P, I64, P, I64, P, P],
+        "xrs_local_combine_scratch_bytes": [I64, I64, ctypes.POINTER(I64)],
+        "xrs_local_combine": [P, I64, P, I64, I64, I, P, I64, P, P, I64, P, P],
         "xrs_host_stencil":[I, P, I, P, I64, I64, P, P, I, P, I],
         "xrs_host_release": [I],
         "xrs_host_alloc": [ctypes.POINTER(P), I64],

@@ -210,6 +210,15 @@ CELL_POLICIES = {
 }
 
 
+def uint64_as_int64(a, what):
+    """The int64 view of uint64 cells (numpy or torch), which is their value when every cell is below 2**63: the
+    others are its negative cells, and raise ValueError."""
+    view = a.view(np.int64) if isinstance(a, np.ndarray) else a.view(torch.int64)
+    if bool((view < 0).any()):
+        raise ValueError("%s: uint64 cells above 2**63 - 1 are not supported" % what)
+    return view
+
+
 def raster_cells(data, what, policy):
     """A numpy or device 2-D raster checked against CELL_POLICIES[policy], as the numpy array or CUDA tensor of the
     cells the entry point reads, and their code.  Nothing is uploaded."""
@@ -227,10 +236,7 @@ def raster_cells(data, what, policy):
     name = str(a.dtype).replace("torch.", "")
     host = isinstance(a, np.ndarray)
     if name == "uint64" and widen.get(name) == "int64":
-        # uint64 cells below 2**63 are their own int64 view; the others are the negative ones of it
-        a, name = a.view(np.int64 if host else torch.int64), "int64"
-        if bool((a < 0).any()):
-            raise ValueError("%s: uint64 cells above 2**63 - 1 are not supported" % what)
+        a, name = uint64_as_int64(a, what), "int64"
     elif name in widen:
         name = widen[name]
         a = a.astype(name) if host else a.to(getattr(torch, name))
