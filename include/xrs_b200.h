@@ -50,9 +50,12 @@ enum xrs_focal_stat {
 
 /* cell types of raster arguments.  Two sets of them:
  *   the raster set, XRS_F32 .. XRS_U16 (codes 0-5): read by proximity, viewshed, a_star_search and classify;
- *   the zonal set, every code (0-10): read by xrs_zonal_regions and xrs_zonal_bounds.
- * A code outside an entry point's set returns XRS_EINVAL ("unknown cell type"); its input pitch must be a multiple
- * of the cell size and at least a row. */
+ *   the zonal set, every code (0-10): read by xrs_zonal_regions, xrs_zonal_bounds and the local entry points.
+ * A code outside an entry point's set returns XRS_EINVAL ("unknown cell type").  The pitched stencils, geodesic
+ * and noise read fixed types of the raster set: float32 (the *_f32 surface, focal and convolution entry points),
+ * float64 (xrs_focal_mean_f64), int16 / uint16 / int32 / float64 (xrs_surface_typed), float32 or float64
+ * (xrs_geodesic, xrs_noise).  For every one of these entry points, an input or output pitch must be a multiple of
+ * the cell size and at least a row ("bad input pitch", "bad output pitch": XRS_EINVAL). */
 enum xrs_dtype { XRS_F32 = 0, XRS_F64 = 1, XRS_I32 = 2, XRS_I64 = 3, XRS_I16 = 4, XRS_U16 = 5,
                  XRS_I8 = 6, XRS_U8 = 7, XRS_U32 = 8, XRS_U64 = 9, XRS_BOOL = 10 };
 

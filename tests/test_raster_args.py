@@ -1,6 +1,7 @@
-"""Raster arguments: the cell sets and argument checks every raster entry point shares (common.cuh), and the one
-Python path from a raster to device cells (utils.device_cells): policies, broadcast rasters, uint64 widening and
-scratch allocation failures."""
+"""Raster arguments: the cell sets and argument checks every raster entry point shares (common.cuh), the stencils'
+pitch checks included, and the one Python path from a raster to device cells (utils.device_cells and
+utils.run_stencil_device): policies, broadcast and transposed rasters, uint64 widening and scratch allocation
+failures."""
 import ctypes
 import importlib
 
@@ -114,6 +115,58 @@ def test_scratch_one_byte_short_is_too_small(name):
         assert entry[3] in _message() and (name == "xrs_a_star_snap" or b"_scratch_bytes)" in _message())
 
 
+_obuf = (ctypes.c_double * 64)()
+Q = ctypes.cast(_obuf, ctypes.c_void_p)   # the output: convolve and the focal statistics check aliasing first
+_K = (ctypes.c_double * 9)(*[1.0] * 9)    # a 3 x 3 window, and the surface operators' parameters
+_STATS = (ctypes.c_int * 1)(0)
+
+
+def _stencils():
+    """name: (input cell code, output cell bytes, call(in, in_pitch, out_pitch)) of the pitched stencil, convolution,
+    focal and geodesic entry points.  Every other argument is valid, so each call stops at the check under test."""
+    L, k, F32, F64 = _lib.lib(), ctypes.cast(_K, ctypes.c_void_p), 0, 1
+    table = {
+        "xrs_slope_f32": (F32, 4, lambda i, ip, op: L.xrs_slope_f32(i, ip, Q, op, H, W, 1.0, 1.0, None)),
+        "xrs_aspect_f32": (F32, 4, lambda i, ip, op: L.xrs_aspect_f32(i, ip, Q, op, H, W, None)),
+        "xrs_curvature_f32": (F32, 4, lambda i, ip, op: L.xrs_curvature_f32(i, ip, Q, op, H, W, 1.0, None)),
+        "xrs_hillshade_f32": (F32, 4, lambda i, ip, op: L.xrs_hillshade_f32(i, ip, Q, op, H, W, 225.0, 25.0, None)),
+        "xrs_surface_suite_f32": (F32, 4, lambda i, ip, op: L.xrs_surface_suite_f32(
+            i, ip, Q, None, None, None, op, H, W, 1.0, 1.0, 225.0, 25.0, None)),
+        "xrs_focal_mean_f32": (F32, 4, lambda i, ip, op: L.xrs_focal_mean_f32(i, ip, Q, op, H, W, None, 0, None)),
+        "xrs_focal_mean_f64": (F64, 8, lambda i, ip, op: L.xrs_focal_mean_f64(i, ip, Q, op, H, W, None, 0, None)),
+        "xrs_focal_mean_f32_f64": (F32, 8, lambda i, ip, op: L.xrs_focal_mean_f32_f64(
+            i, ip, Q, op, H, W, None, 0, None)),
+        "xrs_convolve2d_f32": (F32, 4, lambda i, ip, op: L.xrs_convolve2d_f32(i, ip, Q, op, H, W, k, 3, 3, None)),
+        "xrs_focal_stat_f32": (F32, 4, lambda i, ip, op: L.xrs_focal_stat_f32(i, ip, Q, op, H, W, k, 3, 3, 0, None)),
+        "xrs_focal_stats_multi_f32": (F32, 4, lambda i, ip, op: L.xrs_focal_stats_multi_f32(
+            i, ip, Q, op, 4096, H, W, k, 3, 3, _STATS, 1, None)),
+    }
+    for name in ("int16", "uint16", "int32", "float64"):
+        code = _lib.DTYPES[name]
+        table["xrs_surface_typed " + name] = (code, 4, lambda i, ip, op, code=code: L.xrs_surface_typed(
+            _lib.OPS["slope"], i, code, ip, Q, op, H, W, k, None))
+    for name in ("float32", "float64"):
+        code = _lib.DTYPES[name]
+        table["xrs_geodesic " + name] = (code, 4, lambda i, ip, op, code=code: L.xrs_geodesic(
+            i, code, ip, k, k, 0, Q, op, H, W, 1.0, 0, None))
+    return table
+
+
+@pytest.mark.parametrize("name", sorted(_stencils()))
+def test_stencils_refuse_a_null_input_and_bad_pitches(name):
+    code, osz, call = _stencils()[name]
+    esz = CELL_SIZE[code]
+    row, out_row = _row(code), _row(code, osz)
+    assert call(None, row, out_row) == _lib.XRS_EINVAL
+    assert b"NULL input" in _message(), (name, _message())
+    for ip in [row - esz] + ([row + 1] if esz > 1 else []):
+        assert call(P, ip, out_row) == _lib.XRS_EINVAL
+        assert b"input pitch" in _message(), (name, ip, _message())
+    for op in (out_row - osz, out_row + 1):
+        assert call(P, row, op) == _lib.XRS_EINVAL
+        assert b"output pitch" in _message(), (name, op, _message())
+
+
 # ----------------------------------------------------------------------------- the Python cell policies
 @pytest.mark.parametrize("dtype, widen, as_is, floats", [
     ("float32", "float32", "float32", "float32"), ("float64", "float64", "float64", "float64"),
@@ -170,6 +223,105 @@ def test_broadcast_rasters_give_the_contiguous_result():
                 lambda d: xb.quantile(_da(d), k=3).data, lambda d: xb.regions(_da(d)).data]
         for run in runs:
             _same(run(b), run(c))
+
+
+def _identical(a, b):
+    """a and b (tensors or numpy arrays) hold the same bits."""
+    import torch
+    a, b = (torch.as_tensor(x).cpu().contiguous() for x in (a, b))
+    assert a.dtype == b.dtype and a.shape == b.shape
+    view = {1: torch.int8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[a.element_size()]
+    assert torch.equal(a.view(view), b.view(view))
+
+
+_SURFACE = (xb.slope, xb.aspect, xb.curvature, xb.hillshade)
+_ROW = np.array([0, 0, 3, 0, 5, 5, 0, 2, 0, 1, 0, 0, 4, 7, 1, 9])   # W % 4 == 0: the ingest kernels take it
+
+
+def _broadcast(row, h):
+    """h rows 0 bytes apart, each the 1-D tensor `row` (expand gives a 1-row raster a row stride of W)."""
+    return row.as_strided((h, row.numel()), (0, 1))
+
+
+def _dense(t):
+    """A copy of t with rows a row apart (t.contiguous() returns a 1-row raster of row stride 0 as it is)."""
+    import torch
+    return t.clone(memory_format=torch.contiguous_format)
+
+
+def _derive(d, fn):
+    """fn(d), broadcast as d is (an elementwise op on a broadcast tensor gives a contiguous one)."""
+    return _broadcast(fn(d[0]), d.shape[0]) if d.stride(0) == 0 else fn(d)
+
+
+def _device_calls():
+    """Every device call a float32 raster d can make beside the planar surface operators, as functions of d."""
+    import torch
+    k = np.array([[0, 1, 0], [1, 1, 1], [0, 1, 0]], np.float64)
+    plus = lambda d, c: _da(_derive(d, lambda x: x + c))   # noqa: E731
+    return [lambda d: xb.mean(_da(d)).data, lambda d: xb.mean(_da(_derive(d, lambda x: x.double()))).data,
+            lambda d: xb.convolve_2d(d, k), lambda d: xb.focal_apply(_da(d), k).data,
+            lambda d: xb.focal_stats(_da(d), k).data,
+            lambda d: torch.stack([r.data for r in xb.surface_suite(_da(d)).values()]),
+            lambda d: xb.slope(_da(d), method="geodesic").data,
+            lambda d: xb.ndvi(_da(d), plus(d, 1)).data, lambda d: xb.evi(plus(d, 3), _da(d), plus(d, 1)).data,
+            lambda d: xb.hotspots(_da(d), k).data,
+            lambda d: xb.zonal_stats(_da(_derive(d, lambda x: x.int())), plus(d, 0.5)),
+            lambda d: xb.local.cell_stats(xb.Dataset({"a": d, "b": _derive(d, lambda x: x * 2)})).data]
+
+
+@pytest.mark.gpu
+def test_broadcast_rasters_give_the_contiguous_result_through_every_device_call():
+    import pandas as pd
+    import torch
+    for h in (1, 7):
+        for dt in (np.float32, np.int16, np.uint16, np.int32, np.float64):
+            b = _broadcast(torch.from_numpy(_ROW.astype(dt)).cuda(), h)
+            assert b.stride(0) == 0
+            for f in _SURFACE:
+                _identical(f(_da(b)).data, f(_da(_dense(b))).data)
+        b = _broadcast(torch.from_numpy(_ROW.astype(np.float32)).cuda(), h)
+        for run in _device_calls():
+            got, want = run(b), run(_dense(b))
+            if isinstance(got, pd.DataFrame):
+                pd.testing.assert_frame_equal(got, want, check_exact=True)
+            else:
+                _identical(got, want)
+
+
+@pytest.mark.gpu
+def test_transposed_typed_views_take_the_ingest_kernel_with_the_contiguous_result():
+    import torch
+    from helpers import K_INGEST
+    base = np.random.default_rng(7).integers(-300, 300, (256, 64))
+    for cells in (base.astype(np.int16), base * 1.000000123):
+        t = torch.from_numpy(cells).cuda().T
+        assert t.stride(1) != 1
+        for f in _SURFACE:
+            got = f(_da(t)).data
+            assert _lib.lib().xrs_debug_last_used_tma() == K_INGEST, (f.__name__, t.dtype)
+            _identical(got, f(_da(t.contiguous())).data)
+
+
+@pytest.mark.gpu
+def test_aligned_and_broadcast_int16_rasters_take_the_ingest_kernel():
+    import torch
+    from helpers import K_INGEST
+    a = torch.from_numpy((np.arange(32 * 256).reshape(32, 256) % 23).astype(np.int16)).cuda()
+    for t in (a, a[3].expand(32, 256)):
+        xb.slope(_da(t))
+        assert _lib.lib().xrs_debug_last_used_tma() == K_INGEST
+
+
+@pytest.mark.gpu
+def test_slope_runs_on_the_rasters_device():
+    import torch
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs 2 GPUs")
+    z = torch.from_numpy(np.random.default_rng(3).standard_normal((64, 96)).astype(np.float32))
+    got = xb.slope(_da(z.to("cuda:1"))).data
+    assert got.device == torch.device("cuda:1")
+    _identical(got, xb.slope(_da(z.to("cuda:0"))).data)
 
 
 @pytest.mark.gpu

@@ -1,8 +1,8 @@
 """xrspatial.aspect on the CUDA backend (reference: aspect.py:274-388, planar)."""
 from ._xr import DataArray
 from .dataset_support import supports_dataset
-from .utils import (Z_UNITS, ArrayTypeFunctionMapping, extract_latlon, run_geodesic, run_stencil_host,
-                    run_surface_device)
+from .utils import (Z_UNITS, ArrayTypeFunctionMapping, extract_latlon, run_geodesic, run_stencil_device,
+                    run_stencil_host)
 
 
 def _run_numpy(data):
@@ -12,7 +12,7 @@ def _run_numpy(data):
 
 def _run_cupy(data):
     """replaces aspect.py:139 `_run_cupy`; follows the CPU path (no 359.999 clamp)."""
-    return run_surface_device("aspect", "xrs_aspect_f32", data)
+    return run_stencil_device(data, "xrs_aspect_f32", op="aspect")
 
 
 @supports_dataset

@@ -866,11 +866,11 @@ static bool mask_bits(MaskBits &mask, const double *kernel, int kh, int kw) {
 
 static int check_common(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,
                         const double *kernel, int kh, int kw) {
-    XRS_REQUIRE(in && out && kernel, "NULL pointer");
+    XRS_REQUIRE(out && kernel, "NULL pointer");
     XRS_REQUIRE((const void *)in != (const void *)out, "in and out must not alias");
     if (const int rc = check_window(kh, kw)) return rc;
-    XRS_REQUIRE(in_pitch % 4 == 0 && in_pitch >= W * 4 && out_pitch % 4 == 0 && out_pitch >= W * 4,
-                "pitches must be multiples of 4 bytes and >= row bytes");
+    XRS_TRY(check_cells_arg(in, XRS_F32, kRasterCells, in_pitch, W));
+    XRS_TRY(check_out_pitch(out_pitch, 4, W));
     XRS_REQUIRE(H < (1LL << 31) - 64 && W < (1LL << 31) - 256, "raster dimension too large");
     return XRS_OK;
 }
@@ -935,11 +935,10 @@ static int focal_stats(const float *in, int64_t in_pitch, const StatPlanes &plan
             return launch_tiles(focal_tile_kernel<S>, g, 3, s, S == kAllStats ? kFocalFused : kFocalTiled, tmap,
                                 mask, focal_out<S>(planes), out_pitch / 4, g);
         });
-    const int64_t cell_ctas = (H * W + 255) / 256, max_ctas = (int64_t)sm_count() * 8;
     for (int i = 0; i < 7; ++i) {
         if (!planes.p[i]) continue;
-        const int rc = launch(focal_stat_direct_kernel, cell_ctas < max_ctas ? cell_ctas : max_ctas, 256, 0, s,
-                              kFocalDirect, in, in_pitch / 4, mask, planes.p[i], out_pitch / 4, H, W, kh, kw, i);
+        const int rc = launch(focal_stat_direct_kernel, stride_grid(H * W), 256, 0, s, kFocalDirect, in, in_pitch / 4,
+                              mask, planes.p[i], out_pitch / 4, H, W, kh, kw, i);
         if (rc) return rc;
     }
     return XRS_OK;
@@ -985,9 +984,8 @@ int xrs_convolve2d_f32(const float *in, int64_t in_pitch, float *out, int64_t ou
         }
         return launch_tiles(kern, g, INT_MAX, (cudaStream_t)s, kConvTiled, tmap, cw, out, out_pitch / 4, g);
     }
-    const int64_t cell_ctas = (H * W + 255) / 256, max_ctas = (int64_t)sm_count() * 8;
-    return launch(conv2d_direct_kernel, cell_ctas < max_ctas ? cell_ctas : max_ctas, 256, 0, (cudaStream_t)s,
-                  kConvDirect, in, in_pitch / 4, cw, out, out_pitch / 4, H, W, kh, kw);
+    return launch(conv2d_direct_kernel, stride_grid(H * W), 256, 0, (cudaStream_t)s, kConvDirect, in, in_pitch / 4, cw,
+                  out, out_pitch / 4, H, W, kh, kw);
 }
 
 int xrs_focal_stat_f32(const float *in, int64_t in_pitch, float *out, int64_t out_pitch, int64_t H, int64_t W,

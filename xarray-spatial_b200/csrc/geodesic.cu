@@ -188,11 +188,11 @@ extern "C" int xrs_geodesic(const void *elev, int elev_dtype, int64_t elev_pitch
                             const double *lon, int latlon_2d, float *out, int64_t out_pitch, int64_t H, int64_t W,
                             double z_factor, int want_aspect, xrs_stream_t s) {
     if (H <= 0 || W <= 0) return XRS_OK;
-    XRS_REQUIRE(elev && lat && lon && out, "NULL pointer");
     XRS_REQUIRE(elev_dtype == XRS_F32 || elev_dtype == XRS_F64, "elevation must be float32 or float64");
-    const int esz = elev_dtype == XRS_F32 ? 4 : 8;
-    XRS_REQUIRE(elev_pitch % esz == 0 && elev_pitch >= W * esz, "bad elevation pitch");
-    XRS_REQUIRE(out_pitch % 4 == 0 && out_pitch >= W * 4, "bad output pitch");
+    XRS_TRY(check_cells_arg(elev, elev_dtype, kRasterCells, elev_pitch, W));
+    XRS_REQUIRE(lat && lon && out, "NULL pointer");
+    XRS_TRY(check_out_pitch(out_pitch, 4, W));
+    const int esz = cell_size(elev_dtype);
     cudaStream_t st = (cudaStream_t)s;
     GeoArgs a;
     a.elev = elev; a.pitch_elems = elev_pitch / esz; a.lat = lat; a.lon = lon; a.rt = nullptr; a.ct = nullptr;
@@ -207,9 +207,7 @@ extern "C" int xrs_geodesic(const void *elev, int elev_dtype, int64_t elev_pitch
         geo_tables_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(lat, lon, H, W, rt, ct);
         a.rt = rt; a.ct = ct;
     }
-    int64_t grid = (H * W + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (grid > cap) grid = cap;
+    const int64_t grid = stride_grid(H * W);
     if (elev_dtype == XRS_F32) {
         if (latlon_2d) geodesic_kernel<float, true><<<(unsigned)grid, 256, 0, st>>>(a);
         else geodesic_kernel<float, false><<<(unsigned)grid, 256, 0, st>>>(a);

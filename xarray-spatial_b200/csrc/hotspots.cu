@@ -71,11 +71,7 @@ int xrs_global_stats_f32(const float *values, int64_t n, double pivot, double *p
     XRS_REQUIRE(partial3 != nullptr && (values != nullptr || n == 0), "NULL pointer");
     XRS_CUDA(cudaMemsetAsync(partial3, 0, 3 * sizeof(double), (cudaStream_t)s));
     if (n <= 0) return XRS_OK;
-    int64_t grid = (n / 4 + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (grid > cap) grid = cap;
-    if (grid < 1) grid = 1;
-    global_stats_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)s>>>(values, n, pivot, partial3);
+    global_stats_kernel<<<(unsigned)stride_grid(n / 4), 256, 0, (cudaStream_t)s>>>(values, n, pivot, partial3);
     XRS_CUDA(cudaGetLastError());
     return XRS_OK;
 }
@@ -84,11 +80,8 @@ int xrs_hotspots_classify_f32(const float *mean, int64_t n, double global_mean, 
                               xrs_stream_t s) {
     if (n <= 0) return XRS_OK;
     XRS_REQUIRE(mean && out, "NULL pointer");
-    int64_t grid = (n + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (grid > cap) grid = cap;
-    hotspots_classify_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)s>>>(mean, n, (float)global_mean, (float)global_std,
-                                                                         (signed char *)out);
+    hotspots_classify_kernel<<<(unsigned)stride_grid(n), 256, 0, (cudaStream_t)s>>>(mean, n, (float)global_mean,
+                                                                                   (float)global_std, (signed char *)out);
     XRS_CUDA(cudaGetLastError());
     return XRS_OK;
 }

@@ -93,10 +93,7 @@ static int launch_band(const float *a, const float *b, const float *c, float *ou
     const bool vec = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) |
                        reinterpret_cast<uintptr_t>(c) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
     const int64_t work = vec ? (n + 3) / 4 : n;
-    int64_t grid = (work + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 8;  // 8 resident CTAs of 256 threads per SM
-    if (grid > cap) grid = cap;
-    band_kernel<NIN, F><<<(unsigned)grid, 256, 0, (cudaStream_t)s>>>(a, b, c, out, n, vec ? 1 : 0, f);
+    band_kernel<NIN, F><<<(unsigned)stride_grid(work), 256, 0, (cudaStream_t)s>>>(a, b, c, out, n, vec ? 1 : 0, f);
     XRS_CUDA(cudaGetLastError());
     return XRS_OK;
 }

@@ -599,11 +599,8 @@ int launch_stencil3(const TS *in, int64_t in_pitch_bytes, const typename Op::Par
     using TO = typename Op::out_t;
     constexpr bool kConvert = !std::is_same<TS, T>::value;
     if (H <= 0 || W <= 0) return XRS_OK;  // empty raster: nothing to do
-    XRS_REQUIRE(in != nullptr, "input pointer is NULL");
-    XRS_REQUIRE(in_pitch_bytes % (int64_t)sizeof(TS) == 0 && in_pitch_bytes >= W * (int64_t)sizeof(TS),
-                "input pitch must be a multiple of the element size and >= row bytes");
-    XRS_REQUIRE(out_pitch_bytes % (int64_t)sizeof(TO) == 0 && out_pitch_bytes >= W * (int64_t)sizeof(TO),
-                "output pitch must be a multiple of the element size and >= row bytes");
+    XRS_TRY(check_cells_arg(in, dtype_of<TS>(), kRasterCells, in_pitch_bytes, W));
+    XRS_TRY(check_out_pitch(out_pitch_bytes, sizeof(TO), W));
     XRS_REQUIRE(H < (1LL << 31) - 8 && W < (1LL << 31) - 4096, "raster dimension too large");
 
     OutPtrs<Op> outs;

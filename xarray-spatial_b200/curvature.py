@@ -1,7 +1,7 @@
 """xrspatial.curvature on the CUDA backend (reference: curvature.py:111-247)."""
 from ._xr import DataArray
 from .dataset_support import supports_dataset
-from .utils import ArrayTypeFunctionMapping, get_dataarray_resolution, run_stencil_host, run_surface_device
+from .utils import ArrayTypeFunctionMapping, get_dataarray_resolution, run_stencil_device, run_stencil_host
 
 
 def _run_numpy(data, cellsize):
@@ -11,7 +11,7 @@ def _run_numpy(data, cellsize):
 
 def _run_cupy(data, cellsize):
     """replaces curvature.py:81 `_run_cupy`."""
-    return run_surface_device("curvature", "xrs_curvature_f32", data, cellsize)
+    return run_stencil_device(data, "xrs_curvature_f32", cellsize, op="curvature")
 
 
 @supports_dataset

@@ -14,8 +14,8 @@ from . import _lib
 from ._xr import DataArray, concat
 from .convolution import custom_kernel
 from .dataset_support import supports_dataset
-from .utils import (ArrayTypeFunctionMapping, _dbl_array, as_device_tensor, device_2d, is_device_array,
-                    like_container, run_stencil_device, run_stencil_host, stream_ptr)
+from .utils import (ArrayTypeFunctionMapping, _dbl_array, as_device_tensor, call_on, device_2d, is_device_array,
+                    like_container, pitch, ptr, run_stencil_device, run_stencil_host)
 
 
 class _Reducer(object):
@@ -66,8 +66,8 @@ def _mean_cupy(data, excludes):
     import torch
     ex = _dbl_array(tuple(excludes))
     if as_device_tensor(data).dtype == torch.float64:
-        return run_stencil_device("xrs_focal_mean_f64", data, ex, len(excludes), dtype=torch.float64)
-    return run_stencil_device("xrs_focal_mean_f32", data, ex, len(excludes))
+        return run_stencil_device(data, "xrs_focal_mean_f64", ex, len(excludes), cells=("float64",), out="float64")
+    return run_stencil_device(data, "xrs_focal_mean_f32", ex, len(excludes))
 
 
 def _mean(data, excludes):
@@ -118,7 +118,7 @@ def _apply_numpy(data, kernel, func):
 def _apply_cupy(data, kernel, func):
     """device raster -> xrs_focal_stat_f32 with the CPU (NaN-skipping) semantics."""
     k = np.ascontiguousarray(kernel, dtype=np.float64)
-    return run_stencil_device("xrs_focal_stat_f32", data, k.ctypes.data_as(ctypes.c_void_p), k.shape[0], k.shape[1],
+    return run_stencil_device(data, "xrs_focal_stat_f32", k.ctypes.data_as(ctypes.c_void_p), k.shape[0], k.shape[1],
                               _lib.STATS[_stat_of(func)])
 
 
@@ -146,12 +146,9 @@ def _focal_stats_cupy(data, kernel, stats_funcs):
     plane = (H * W + 3) // 4 * 4          # planes start on 16-byte boundaries
     out = torch.empty(len(stats_funcs) * plane, dtype=torch.float32, device=t.device)
     out = out.as_strided((len(stats_funcs), H, W), (plane, W, 1))
-    if H and W:
-        with torch.cuda.device(t.device):
-            _lib.call("xrs_focal_stats_multi_f32", ctypes.c_void_p(t.data_ptr()), t.stride(0) * 4,
-                      ctypes.c_void_p(out.data_ptr()), out.stride(1) * 4, out.stride(0) * 4, H, W,
-                      k.ctypes.data_as(ctypes.c_void_p), k.shape[0], k.shape[1], ids, len(stats_funcs),
-                      stream_ptr(t))
+    if H and W:   # the row and the plane pitch of the stack
+        call_on(t, "xrs_focal_stats_multi_f32", ptr(t), pitch(t), ptr(out), pitch(out[0]), pitch(out), H, W,
+                k.ctypes.data_as(ctypes.c_void_p), k.shape[0], k.shape[1], ids, len(stats_funcs))
     return like_container(out, data)
 
 
@@ -195,9 +192,7 @@ def _hotspots_device(data, kernel):
     sample = flat[::step]
     sample = sample[~torch.isnan(sample)]
     pivot = float(sample.double().mean().item()) if sample.numel() else 0.0
-    with torch.cuda.device(t.device):
-        _lib.call("xrs_global_stats_f32", ctypes.c_void_p(tc.data_ptr()), tc.numel(), pivot,
-                  ctypes.c_void_p(part.data_ptr()), stream_ptr(tc))
+    call_on(tc, "xrs_global_stats_f32", ptr(tc), tc.numel(), pivot, ptr(part))
     cnt, s1, s2 = [float(x) for x in part.cpu().numpy()]
     if cnt == 0:
         gmean = gstd = float("nan")
@@ -208,9 +203,8 @@ def _hotspots_device(data, kernel):
         raise ZeroDivisionError("Standard deviation of the input raster values is 0.")
     out = torch.empty(tuple(t.shape), dtype=torch.int8, device=t.device)
     m = mean_array.contiguous()
-    with torch.cuda.device(t.device):
-        _lib.call("xrs_hotspots_classify_f32", ctypes.c_void_p(m.data_ptr()), m.numel(), float(np.float32(gmean)),
-                  float(np.float32(gstd)), ctypes.c_void_p(out.data_ptr()), stream_ptr(m))
+    call_on(m, "xrs_hotspots_classify_f32", ptr(m), m.numel(), float(np.float32(gmean)), float(np.float32(gstd)),
+            ptr(out))
     return out
 
 

@@ -1,9 +1,7 @@
 """xrspatial.hillshade on the CUDA backend (reference: hillshade.py:103-208, shadows=False)."""
-import numpy as np
-
 from ._xr import DataArray
 from .dataset_support import supports_dataset
-from .utils import is_dask_array, is_device_array, run_stencil_host, run_surface_device
+from .utils import ArrayTypeFunctionMapping, run_stencil_device, run_stencil_host
 
 
 def _run_numpy(data, azimuth=225, angle_altitude=25):
@@ -15,7 +13,7 @@ def _run_numpy(data, azimuth=225, angle_altitude=25):
 
 def _run_cupy(d_data, azimuth, angle_altitude):
     """replaces hillshade.py:78 `_run_cupy`."""
-    return run_surface_device("hillshade", "xrs_hillshade_f32", d_data, azimuth, angle_altitude)
+    return run_stencil_device(d_data, "xrs_hillshade_f32", azimuth, angle_altitude, op="hillshade")
 
 
 @supports_dataset
@@ -23,12 +21,6 @@ def hillshade(agg, azimuth=225, angle_altitude=25, name='hillshade', shadows=Fal
     """Illumination in [0, 1] from (azimuth, angle_altitude); NaN ring."""
     if shadows:
         raise RuntimeError("Can only calculate shadows if cupy and rtxpy are available")
-    if isinstance(agg.data, np.ndarray):
-        out = _run_numpy(agg.data, azimuth, angle_altitude)
-    elif is_device_array(agg.data):
-        out = _run_cupy(agg.data, azimuth, angle_altitude)
-    elif is_dask_array(agg.data):
-        raise NotImplementedError("dask-backed DataArrays are not supported by the CUDA backend")
-    else:
-        raise TypeError('Unsupported Array Type: {}'.format(type(agg.data)))
+    mapper = ArrayTypeFunctionMapping(numpy_func=_run_numpy, cupy_func=_run_cupy)
+    out = mapper(agg)(agg.data, azimuth, angle_altitude)
     return DataArray(out, name=name, coords=agg.coords, dims=agg.dims, attrs=agg.attrs)

@@ -12,7 +12,7 @@ import numpy as np
 
 from . import _lib
 from ._xr import DataArray, Dataset
-from .utils import device_2d, device_scratch, raster_cells, stream_ptr, uint64_as_int64
+from .utils import call_on, device_2d, device_scratch, pitch, ptr, raster_cells, uint64_as_int64
 
 try:
     import torch
@@ -104,7 +104,7 @@ class _Stack:
     def descriptors(self, tensors):
         """K layers as the host array {pointer, pitch, dtype} per layer the entry points take, and a device
         buffer for their copy."""
-        rows = [(t.data_ptr(), t.stride(0) * t.element_size(), c) for t, c in zip(tensors, self.codes)]
+        rows = [(t.data_ptr(), pitch(t), c) for t, c in zip(tensors, self.codes)]
         host = (ctypes.c_int64 * (3 * len(rows)))(*[v for r in rows for v in r])
         return host, torch.empty(3 * len(rows), dtype=torch.int64, device=self.device)
 
@@ -148,14 +148,10 @@ def _run(op, raster, data_vars, ref_var=None):
     if H and W:
         host, dev = s.descriptors(s.tensors[:s.K])
         ref = s.tensors[s.K] if ref_var is not None else None
-        with torch.cuda.device(s.device):
-            _lib.call("xrs_local_cells", host, s.K, ctypes.c_void_p(dev.data_ptr()), H, W, op, s.ak,
-                      ctypes.c_void_p(ref.data_ptr() if ref is not None else 0),
-                      ref.stride(0) * ref.element_size() if ref is not None else 0,
-                      s.codes[s.K] if ref is not None else 0, int(ref is not None and s.f16[s.K]),
-                      ctypes.c_void_p(bits.data_ptr()), W * 8,
-                      ctypes.c_void_p(kinds.data_ptr() if kinds is not None else 0), W,
-                      ctypes.c_void_p(flags.data_ptr()), stream_ptr(bits))
+        call_on(bits, "xrs_local_cells", host, s.K, ptr(dev), H, W, op, s.ak, None if ref is None else ptr(ref),
+                0 if ref is None else pitch(ref), 0 if ref is None else s.codes[s.K],
+                int(ref is not None and s.f16[s.K]), ptr(bits), pitch(bits), None if kinds is None else ptr(kinds), W,
+                ptr(flags))
     out = _finish(op, s.ak, bits, kinds, int(flags.item()), _ref_type(s) if ref_var is not None else None)
     return DataArray(s.container(out))
 
@@ -178,17 +174,13 @@ def _combine(raster, data_vars):
         host, dev = s.descriptors(s.tensors)
         scratch, nbytes = device_scratch("xrs_local_combine_scratch_bytes", H, W, device=s.device, what="combine")
         table = scratch[:nbytes].view(torch.int64)
-        args = [host, s.K, ctypes.c_void_p(dev.data_ptr()), H, W]
-        with torch.cuda.device(s.device):
-            _lib.call("xrs_local_combine", *args, 0, ctypes.c_void_p(scratch.data_ptr()), nbytes, None,
-                      ctypes.c_void_p(ids.data_ptr()), W * 8, ctypes.c_void_p(flags.data_ptr()), stream_ptr(ids))
-            # the occupied slots hold each tuple's first cell: number them in that order
-            slots = torch.nonzero(table != torch.iinfo(torch.int64).max).flatten()
-            reps, order = torch.sort(table[slots])
-            table[slots[order]] = -1 - torch.arange(len(reps), device=s.device)
-            _lib.call("xrs_local_combine", *args, 1, ctypes.c_void_p(scratch.data_ptr()), nbytes,
-                      ctypes.c_void_p(reps.data_ptr()), ctypes.c_void_p(ids.data_ptr()), W * 8,
-                      ctypes.c_void_p(flags.data_ptr()), stream_ptr(ids))
+        args = [host, s.K, ptr(dev), H, W]
+        call_on(ids, "xrs_local_combine", *args, 0, ptr(scratch), nbytes, None, ptr(ids), pitch(ids), ptr(flags))
+        # the occupied slots hold each tuple's first cell: number them in that order
+        slots = torch.nonzero(table != torch.iinfo(torch.int64).max).flatten()
+        reps, order = torch.sort(table[slots])
+        table[slots[order]] = -1 - torch.arange(len(reps), device=s.device)
+        call_on(ids, "xrs_local_combine", *args, 1, ptr(scratch), nbytes, ptr(reps), ptr(ids), pitch(ids), ptr(flags))
         rows, cols = reps // W, reps % W
         columns = [_gather(t, code, rows, cols) for t, code in zip(s.tensors, s.codes)]
         key = {i + 1: tup for i, tup in enumerate(zip(*columns))}

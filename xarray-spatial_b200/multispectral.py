@@ -9,11 +9,9 @@ import ctypes
 
 import numpy as np
 
-from . import _lib
 from ._xr import DataArray
 from .dataset_support import supports_dataset_bands
-from .utils import (ArrayTypeFunctionMapping, as_device_tensor, like_container, stream_ptr,
-                    validate_arrays)
+from .utils import ArrayTypeFunctionMapping, as_device_tensor, call_on, like_container, ptr, validate_arrays
 
 
 def _band_device(fn_name, bands, scalars=()):
@@ -28,11 +26,8 @@ def _band_device(fn_name, bands, scalars=()):
     out = torch.empty(ts[0].shape, dtype=torch.float32, device=ts[0].device)
     n = out.numel()
     if n:
-        args = [ctypes.c_void_p(t.data_ptr()) for t in ts]
-        args += [s if isinstance(s, ctypes.c_int) else float(s) for s in scalars]
-        args += [ctypes.c_void_p(out.data_ptr()), n]
-        with torch.cuda.device(out.device):
-            _lib.call(fn_name, *args, stream_ptr(out))
+        call_on(out, fn_name, *map(ptr, ts), *[s if isinstance(s, ctypes.c_int) else float(s) for s in scalars],
+                ptr(out), n)
     return like_container(out, bands[0])
 
 

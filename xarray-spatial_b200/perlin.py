@@ -20,7 +20,7 @@ import operator
 import numpy as np
 
 from ._xr import DataArray
-from .utils import call_on, device_2d, device_scratch, host_device_index, is_dask_array, ptr, raster_cells
+from .utils import call_on, device_2d, device_scratch, host_device_index, is_dask_array, pitch, ptr, raster_cells
 from .utils import to_container
 
 TABLE_N = 2 ** 20          # the reference's permutation(2**20)
@@ -85,24 +85,22 @@ def run_noise(data, seeds, xs, ys, terrain, zfactor=0.0):
     H, W = data.shape
     dtype = torch.float32 if str(data.dtype).endswith("float32") else torch.float64
     code = 0 if dtype == torch.float32 else 1
-    with torch.cuda.device(device):
-        tables = perm_tables(seeds, device)
-        dx = torch.from_numpy(np.ascontiguousarray(xs, dtype=np.float32)).to(device)
-        dy = torch.from_numpy(np.ascontiguousarray(ys, dtype=np.float32)).to(device)
-        scratch, size = device_scratch("xrs_noise_scratch_bytes", H, W, int(terrain), device=device,
-                                       what="the noise of a %d x %d raster" % (H, W))
-        try:
-            out = torch.empty((H, W), dtype=dtype, device=device)
-        except torch.OutOfMemoryError as e:
-            raise MemoryError("the noise of a %d x %d raster needs %d bytes of device memory"
-                              % (H, W, H * W * (4 if code == 0 else 8))) from e
-        stats = torch.empty((len(seeds), 5), dtype=torch.int32, device=device)
-        esz = out.element_size()
-        call_on(out, "xrs_noise", ptr(t) if t is not None else None, code, t.stride(0) * esz if t is not None else 0,
-                H, W, ptr(tables), ptr(dx), ptr(dy), int(terrain), float(zfactor), ptr(out), out.stride(0) * esz,
-                ptr(stats), ptr(scratch), size)
-        if index_out_of_range(stats.cpu().numpy()):
-            raise IndexError("index out of bounds for the permutation table of size %d" % INDEX_LIMIT)
+    tables = perm_tables(seeds, device)
+    dx = torch.from_numpy(np.ascontiguousarray(xs, dtype=np.float32)).to(device)
+    dy = torch.from_numpy(np.ascontiguousarray(ys, dtype=np.float32)).to(device)
+    scratch, size = device_scratch("xrs_noise_scratch_bytes", H, W, int(terrain), device=device,
+                                   what="the noise of a %d x %d raster" % (H, W))
+    try:
+        out = torch.empty((H, W), dtype=dtype, device=device)
+    except torch.OutOfMemoryError as e:
+        raise MemoryError("the noise of a %d x %d raster needs %d bytes of device memory"
+                          % (H, W, H * W * (4 if code == 0 else 8))) from e
+    stats = torch.empty((len(seeds), 5), dtype=torch.int32, device=device)
+    call_on(out, "xrs_noise", ptr(t) if t is not None else None, code, pitch(t) if t is not None else 0, H, W,
+            ptr(tables), ptr(dx), ptr(dy), int(terrain), float(zfactor), ptr(out), pitch(out), ptr(stats), ptr(scratch),
+            size)
+    if index_out_of_range(stats.cpu().numpy()):
+        raise IndexError("index out of bounds for the permutation table of size %d" % INDEX_LIMIT)
     return to_container(out, data)
 
 

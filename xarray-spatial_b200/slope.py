@@ -2,7 +2,7 @@
 from ._xr import DataArray
 from .dataset_support import supports_dataset
 from .utils import (Z_UNITS, ArrayTypeFunctionMapping, extract_latlon, get_dataarray_resolution,
-                    run_geodesic, run_stencil_host, run_surface_device)
+                    run_geodesic, run_stencil_device, run_stencil_host)
 
 
 def _run_numpy(data, cellsize_x, cellsize_y):
@@ -12,7 +12,7 @@ def _run_numpy(data, cellsize_x, cellsize_y):
 
 def _run_cupy(data, cellsize_x, cellsize_y):
     """Device raster -> xrs_slope_f32 (replaces slope.py:145 `_run_cupy`)."""
-    return run_surface_device("slope", "xrs_slope_f32", data, cellsize_x, cellsize_y)
+    return run_stencil_device(data, "xrs_slope_f32", cellsize_x, cellsize_y, op="slope")
 
 
 @supports_dataset

@@ -288,44 +288,42 @@ def coord(raster, name):
     return np.asarray(getattr(c, "data", c))
 
 
-def run_stencil_device(fn_name, data, *args, dtype=None):
-    """Call the device entry point `fn_name(in, in_pitch, out, out_pitch, H, W, *args, stream)` on
-    torch's current stream, `args` being its own arguments in header order.  The raster is cast to
-    `dtype` (default float32) and the result has the same dtype."""
-    t = device_2d(data, dtype or torch.float32)
-    H, W = t.shape
-    out = torch.empty((H, W), dtype=t.dtype, device=t.device)
-    if H == 0 or W == 0:
-        return like_container(out, data)
-    esz = t.element_size()
-    with torch.cuda.device(t.device):
-        _lib.call(fn_name, ctypes.c_void_p(t.data_ptr()), t.stride(0) * esz, ctypes.c_void_p(out.data_ptr()),
-                  out.stride(0) * esz, H, W, *args, stream_ptr(t))
-    return like_container(out, data)
-
-
 _SURFACE_OPS = ("slope", "aspect", "curvature", "hillshade")
 _SURFACE_CELLS = ("int16", "uint16", "int32", "float64")   # what the direct-ingest kernels read
 
 
-def run_surface_device(op, fn_name, data, *scalars):
-    """slope / aspect / curvature / hillshade on a device raster.  int16 / uint16 / int32 / float64
-    rasters go through the direct-ingest kernels (xrs_surface_typed: no separate cast pass); other
-    dtypes are cast to float32 first, like the reference does (slope.py:150)."""
-    t = as_device_tensor(data)
-    cells = str(t.dtype).replace("torch.", "")
-    if cells in _SURFACE_CELLS and t.dim() == 2 and t.numel() and t.stride(1) == 1:
-        H, W = t.shape
-        out = torch.empty((H, W), dtype=torch.float32, device=t.device)
-        try:
-            with torch.cuda.device(t.device):
-                _lib.call("xrs_surface_typed", _lib.OPS[op], ctypes.c_void_p(t.data_ptr()), _lib.DTYPES[cells],
-                          t.stride(0) * t.element_size(), ctypes.c_void_p(out.data_ptr()), out.stride(0) * 4, H, W,
-                          _dbl_array(scalars), stream_ptr(t))
-            return like_container(out, data)
-        except NotImplementedError:
-            pass  # layout the ingest kernels do not take (odd width, misaligned rows): cast instead
-    return run_stencil_device(fn_name, data, *[float(s) for s in scalars])
+def run_stencil_device(data, entry, *args, cells=("float32",), out="float32", op=None):
+    """`entry(in, in_pitch, out, out_pitch, H, W, *args, stream)`, a pitched stencil, on the numpy or device raster
+    `data` and torch's current stream: the H x W result of `out` cells, in data's container (an empty raster gets it
+    without a call).
+
+    The raster goes through device_2d (a broadcast or strided one is copied once), then is cast to cells[0] unless
+    its cells are one of `cells` (float32 by default, the reference's `astype`, slope.py:150).  With `op` (slope,
+    aspect, curvature or hillshade, `args` its parameters), int16, uint16, int32 and float64 rasters go to
+    xrs_surface_typed as they are, and are cast only when it refuses their layout.  A callable `entry` is called as
+    entry(cells, result) and makes a call of its own argument layout (run_geodesic)."""
+    t = device_2d(data)
+    H, W = t.shape
+    res = torch.empty((H, W), dtype=getattr(torch, out), device=t.device)
+    if H == 0 or W == 0:
+        return to_container(res, data)
+    name = str(t.dtype).replace("torch.", "")
+    if op is not None:
+        args = [float(s) for s in args]
+        if name in _SURFACE_CELLS:
+            try:
+                call_on(t, "xrs_surface_typed", _lib.OPS[op], ptr(t), _lib.DTYPES[name], pitch(t), ptr(res),
+                        pitch(res), H, W, _dbl_array(args))
+                return to_container(res, data)
+            except NotImplementedError:
+                pass  # a layout the ingest kernels do not take (odd width, misaligned rows): cast instead
+    if name not in cells:
+        t = t.to(getattr(torch, cells[0]))
+    if callable(entry):
+        entry(t, res)
+    else:
+        call_on(t, entry, ptr(t), pitch(t), ptr(res), pitch(res), H, W, *args)
+    return to_container(res, data)
 
 
 def run_stencil_host(op, data, p=(), aux=()):
@@ -420,20 +418,11 @@ def extract_latlon(agg):
 
 
 def run_geodesic(data, lat, lon, is_2d, z_factor, want_aspect):
-    """xrs_geodesic on a device or host raster; result in the container type of `data`."""
-    t = device_2d(data)
-    if t.dtype not in (torch.float32, torch.float64):
-        t = t.to(torch.float64)           # the reference computes on data.astype(float64), slope.py:169
-    H, W = t.shape
-    out = torch.empty((H, W), dtype=torch.float32, device=t.device)
-    if H and W:
-        lat_t = torch.as_tensor(lat, dtype=torch.float64, device=t.device).contiguous()
-        lon_t = torch.as_tensor(lon, dtype=torch.float64, device=t.device).contiguous()
-        with torch.cuda.device(t.device):
-            _lib.call("xrs_geodesic", ctypes.c_void_p(t.data_ptr()), 0 if t.dtype == torch.float32 else 1,
-                      t.stride(0) * t.element_size(), ctypes.c_void_p(lat_t.data_ptr()),
-                      ctypes.c_void_p(lon_t.data_ptr()), 1 if is_2d else 0, ctypes.c_void_p(out.data_ptr()),
-                      out.stride(0) * 4, H, W, float(z_factor), 1 if want_aspect else 0, stream_ptr(t))
-    if isinstance(data, np.ndarray):
-        return out.cpu().numpy()
-    return like_container(out, data)
+    """xrs_geodesic on a numpy or device raster through run_stencil_device; float32 and float64 cells are read as
+    they are, others as float64 (the reference computes on data.astype(float64), slope.py:169)."""
+    def entry(t, res):
+        lat_t, lon_t = (torch.as_tensor(a, dtype=torch.float64, device=t.device).contiguous() for a in (lat, lon))
+        code = _lib.DTYPES[str(t.dtype).replace("torch.", "")]
+        call_on(t, "xrs_geodesic", ptr(t), code, pitch(t), ptr(lat_t), ptr(lon_t), int(is_2d), ptr(res), pitch(res),
+                *t.shape, float(z_factor), int(want_aspect))
+    return run_stencil_device(data, entry, cells=("float64", "float32"))

@@ -16,7 +16,7 @@ import pandas as pd
 from . import _lib
 from ._xr import DataArray, Dataset
 from .utils import (ArrayTypeFunctionMapping, as_device_tensor, call_on, device_cells, device_scratch, like_container,
-                    pitch, ptr, stream_ptr, to_container, validate_arrays)
+                    pitch, ptr, to_container, validate_arrays)
 
 _DEFAULT_STATS = ("mean", "max", "min", "sum", "std", "var", "count", "majority")
 
@@ -117,12 +117,11 @@ def _table_pass(entry, zones_t, values_t, nodata_values, table_args, keys, acc, 
     dt = lambda t: _lib.DTYPES[str(t.dtype).replace("torch.", "")]  # noqa: E731
     packed = torch.empty(_HDR + 6 * _MAX_OUT, dtype=torch.float64, device=values_t.device)
     flags = torch.empty(3, dtype=torch.int32, device=values_t.device)
-    with torch.cuda.device(values_t.device):
-        _lib.call(entry, ptr(values_t), dt(values_t), ptr(zones_t), dt(zones_t), values_t.numel(),
-                  int(values_t.shape[-1]) if values_t.dim() else 1,
-                  0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
-                  *(ptr(a) if torch.is_tensor(a) else a for a in table_args), *(ptr(r) for r in acc),
-                  keys.numel(), ptr(packed), _MAX_OUT, ptr(flags), stream_ptr(values_t))
+    call_on(values_t, entry, ptr(values_t), dt(values_t), ptr(zones_t), dt(zones_t), values_t.numel(),
+            int(values_t.shape[-1]) if values_t.dim() else 1,
+            0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
+            *(ptr(a) if torch.is_tensor(a) else a for a in table_args), *(ptr(r) for r in acc),
+            keys.numel(), ptr(packed), _MAX_OUT, ptr(flags))
     host = packed.cpu().numpy()                    # the one synchronising copy
     n_used, overflow, pivot, sentinel = int(host[0]), int(host[1]), float(host[2]), int(host[3])
     if overflow:
@@ -273,10 +272,9 @@ def pair_counts(zones_t, values_t, nodata_values=None, comm=None, cap=None, max_
         keys = torch.empty(cap, dtype=torch.int64, device=dev)
         count = torch.empty(cap, dtype=torch.int64, device=dev)
         ovf = torch.empty(1, dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.call("xrs_zonal_pair_count", ptr(vf), ptr(zi), vf.numel(), int(vf.shape[-1]) if vf.dim() else 1,
-                      0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
-                      ptr(keys), ptr(count), cap, ptr(ovf), stream_ptr(vf))
+        call_on(vf, "xrs_zonal_pair_count", ptr(vf), ptr(zi), vf.numel(), int(vf.shape[-1]) if vf.dim() else 1,
+                0 if nodata_values is None else 1, 0.0 if nodata_values is None else float(nodata_values),
+                ptr(keys), ptr(count), cap, ptr(ovf))
         if int(ovf.item()) == 0:
             break
         if cap >= max_cap:
